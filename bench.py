@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark: ResNet-18 synchronous parameter-server SGD, samples/sec on N B200s.
+"""Headline benchmark: ResNet-18 synchronous parameter-server SGD, samples/sec on N H100s.
 
 ``python bench.py --gpus N --steps K --warmup W`` (N > 1 under ``torch.distributed.run``).
 Metric / config are BASELINE.json's: "samples/sec (whole box, device-timed, max over ranks) for
@@ -22,9 +22,13 @@ reference-equivalent host comparators in the same invocation (same box, same mod
 prints ``vs_comparator`` / ``comparators`` so every record carries a same-run ratio (``--no-comparators`` skips them).
 
 Timing: W (>= 3) warm-up steps, then warm-up continues until 5 consecutive steps agree within 2 % (clocks ramped, allocator
-settled; at most ~3 s), then EXACTLY K steps between ``barrier + synchronize`` on both sides, one CUDA event per step
+settled; at most ~3 s; exactly W steps with ``--dump-outputs``), then EXACTLY K steps between ``barrier + synchronize`` on both sides, one CUDA event per step
 (total = first → last event; median / p90 of the per-step times are reported too), max over ranks.  SM clocks and
 throttle reasons are read from NVML in-process (a 25 ms polling thread; no child process inside the timed region).
+
+``--dump-outputs DIR`` (rank 0): after the K timed steps, the last step's ``loss.npy`` and ``params.npy`` (every parameter
+after the update, flat in ``named_parameters()`` order, float32; above ``DUMP_MAX_ELEMS`` a seeded sample of ``DUMP_SAMPLE``,
+indices in ``params_index.npy``; at most 48 MB in all).  Inputs and step counts depend only on the arguments, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -62,11 +66,13 @@ def parse():
     ap.add_argument("--no-comparators", action="store_true", help="skip the same-invocation NCCL-PS / host comparators")
     ap.add_argument("--no-pipeline", action="store_true", help="one fused update launch inside step() (round-1 behaviour)")
     ap.add_argument("--profile", action="store_true", help="CUDA-event section timings of the PS path (stderr)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss and updated parameters as .npy files into DIR (rank 0)")
     return ap.parse_args()
 
 
 def reference_unavailable():
-    why = ("reference is not installable: /root/reference has no setup.py/pyproject.toml (pip: 'not installable'), "
+    why = ("reference is not installable: it has no setup.py/pyproject.toml (pip: 'not installable'), "
            "its deps mpi4py/blosc/toolz/distributed/codings are absent offline, and mpi_comms.py:50 "
            "(d.cuda(async=True)) is a SyntaxError on Python 3.12")
     if os.environ.get("RANK", "0") == "0":          # under torchrun only rank 0 reports
@@ -87,6 +93,23 @@ def make_code(ps, name):
     raise ValueError(name)
 
 
+DUMP_MAX_ELEMS = 12 << 20          # parameter vectors up to 48 MB of float32 are written whole
+DUMP_SAMPLE = 4 << 20              # larger ones: 16 MB of sampled float32 values + 32 MB of their float64 indices
+
+
+def dump_outputs(out_dir, model, loss):
+    """The last timed step's results as .npy files (see the module docstring); at most 48 MB + 4 bytes in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss.detach())], dtype=np.float32))
+    flat = torch.cat([p.detach().float().flatten() for _, p in model.named_parameters()]).cpu()
+    if flat.numel() > DUMP_MAX_ELEMS:
+        idx = torch.randint(flat.numel(), (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(0)).unique()
+        flat = flat[idx]
+        np.save(os.path.join(out_dir, "params_index.npy"), idx.double().numpy())
+    np.save(os.path.join(out_dir, "params.npy"), flat.numpy())
+
+
 def build(args, device, ps):
     from pytorch_ps_mpi_b200 import models
     torch.manual_seed(0)
@@ -105,8 +128,6 @@ def build(args, device, ps):
         from pytorch_ps_mpi_b200.ops.preprocess import normalize_nhwc
 
         def loss_fn(x, y):
-            # (the 8-channel padded stem of ops.preprocess.normalize_pad8 measured SLOWER under cuDNN on B200:
-            #  3.45 ms vs 2.51 ms fwd+wgrad — scratch/stem_bench.py — so the stock 3-channel stem stays)
             xb = normalize_nhwc(x)          # uint8 NCHW → normalised bf16 NHWC: one kernel of ours
             return torch.nn.functional.cross_entropy(model(xb).float(), y)
         cfg = {"global_batch": None, "image": "3x224x224 uint8"}
@@ -152,14 +173,17 @@ def main():
     device = w.device
     # one process per GPU: run on the GPU's own socket, so the pinned input batches below are allocated NUMA-locally
     numa = ps.runtime.bind_to_gpu_numa_node(device)
-    torch.backends.cudnn.benchmark = True
+    # the same cuDNN algorithms in every run (no autotuning, deterministic kernels): equal arguments give equal results and time
+    # the same code, instead of whichever algorithm won a noisy timing race in this run
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True
     model, make_batch, loss_fn, cfg = build(args, device, ps)
     K, W = args.steps, max(args.warmup, 3)
     if args.bcast_gemm == "auto":
         args.bcast_gemm = "gate" if args.model in ("resnet18", "resnet50") else "off"
 
-    # one-time setup, not training steps: cuDNN autotuning (cudnn.benchmark) and caching-allocator growth
-    # happen on the first forward/backward of every shape, so run it before the optimizer exists
+    # one-time setup, not training steps: cuDNN plan creation and caching-allocator growth happen on the first
+    # forward/backward of every shape, so run it before the optimizer exists
     if args.model != "mlp":
         gen0 = torch.Generator().manual_seed(7)
         xb, yb = (t.to(device) for t in make_batch(gen0))
@@ -200,7 +224,7 @@ def main():
 
     server_only = args.mode == "async" and w.size > 1 and w.rank == 0   # AsySG-InCon: rank 0 only serves
     zero = torch.zeros((), device=device)
-    state = {"opt": opt}
+    state = {"opt": opt, "loss": zero}
 
     def train_step(x, y):
         o = state["opt"]
@@ -211,6 +235,7 @@ def main():
         loss = loss_fn(x, y)
         loss.backward()
         o.step()
+        state["loss"] = loss
         return loss
 
     def barrier_sync():
@@ -266,12 +291,19 @@ def main():
     with sampler as clk:
         if not clk.ok:                        # no pynvml: fall back to the nvidia-smi child (started before the warm-up)
             clk = ClockSampler(device.index or 0).__enter__()
-        warm_done, stable = stabilise(dev_step, W)
+        if args.dump_outputs:                 # a fixed step count: the dumped state depends on the arguments only
+            timed(W, dev_step)
+            warm_done, stable = W, None
+        else:
+            warm_done, stable = stabilise(dev_step, W)
         clk.mark()
         # ---- arm 1: device-resident inputs (kernel/step time) ----
         launches0 = _ext.cuda().launch_count()
         ms, per = timed(K, dev_step)
         launches = _ext.cuda().launch_count() - launches0      # every psb_* kernel launched in the timed region (C++ counter)
+        if args.dump_outputs and w.rank == 0:
+            torch.cuda.synchronize(device)                      # the last update may run on the engine's side stream
+            dump_outputs(args.dump_outputs, model, state["loss"])
         runs_ms = [ms]
 
         # ---- arm 2: end to end through the public API: H2D of the step's inputs (pinned) + D2H of the loss ----
@@ -302,7 +334,7 @@ def main():
 
             # Default input path: two STATIC device buffers per input, filled alternately by the copy stream from the pinned
             # host batches — what a prefetching data loader does.  No per-step device allocation and no record_stream (the
-            # allocating path above cost 0.5 ms/step at N = 8 against 0.03 ms at N = 1: profiles/bench_r2_n8.json).
+            # allocating path above costs far more per step at N = 8 than at N = 1).
             in_bufs = [tuple(torch.empty(t.shape, dtype=t.dtype, device=device) for t in host[0]) for _ in range(2)]
             copied = [torch.cuda.Event() for _ in range(2)]       # H2D into buffer k finished (copy stream)
             consumed = [torch.cuda.Event() for _ in range(2)]     # the step that read buffer k finished (compute stream)
@@ -433,7 +465,7 @@ def main():
             "config": {"model": args.model, "global_batch": global_batch, "per_gpu_batch": args.batch,
                        "seq_len": cfg.get("seq_len"), "parallelism": f"dp{w.size} (rank-0 parameter server, mode={args.mode})",
                        "optimizer": args.optim, "coding": args.code, "bcast_gemm": args.bcast_gemm, "memory_format": "channels_last",
-                       "l2": "inputs larger than L2: 4 rotating input batches; per-step activations+weights >> 126 MB, no explicit flush",
+                       "l2": "inputs larger than L2: 4 rotating input batches; per-step activations+weights >> 50 MB, no explicit flush",
                        "symmetric_memory": getattr(getattr(eng, "arena", None), "provider", None),
                        "multicast": bool(getattr(getattr(eng, "arena", None), "has_multicast", False)),
                        "bcast": {0: "local", 1: "unicast-p2p", 2: "multimem.st"}.get(getattr(eng, "bcast", -1)),

@@ -15,11 +15,11 @@ vector is many tensors), so the device engine's per-chunk pipeline is on the mea
 
 Reported per size: µs per round trip, gather "bus" GB/s = (N-1)·B_wire / t (what a naive PS's server ingress would
 need), broadcast GB/s = B_param / t, and the fraction of the NVLink roofline
-``max((N-1)·B_wire, B_param) / BW`` for BW = 770 GB/s (measured peer-copy rate per direction, ``B200_PROFILING.md``)
-and BW = 900 GB/s (the nominal figure BASELINE.json quotes).  A fraction above 1 means the switch reduced
+``max((N-1)·B_wire, B_param) / BW`` for BW = the peer-copy rate measured in the same run with ``--peer-copy``, else
+450 GB/s (H100 SXM NVLink 4 per direction, data sheet); ``roofline_source`` says which.  A fraction above 1 means the switch reduced
 (``multimem.ld_reduce``: server ingress is 1×, not (N-1)×).  One JSON line per (size, impl) on rank 0.
 
-    python -m torch.distributed.run --nproc-per-node 8 bench/bandwidth_sweep.py --max-mb 1024 --out profiles/bw_sweep_n8.json
+    python -m torch.distributed.run --nproc-per-node 8 bench/bandwidth_sweep.py --max-mb 1024 --peer-copy --out bw_sweep_n8.json
 """
 from __future__ import annotations
 
@@ -35,8 +35,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import pytorch_ps_mpi_b200 as ps   # noqa: E402
 
-NVLINK_MEASURED_GBS = 770.0     # peer copy per direction per GPU (B200_PROFILING.md; re-measured by --peer-copy)
-NVLINK_NOMINAL_GBS = 900.0      # BASELINE.json
+NVLINK_DATASHEET_GBS = 450.0    # H100 SXM NVLink 4, per direction per GPU (data sheet); --peer-copy measures it instead
 
 
 def timed(w, device, fn, iters, warm=3):
@@ -106,8 +105,11 @@ def main():
         sizes.append(int(b))
         b *= 4
     rows = []
+    link_gbs, link_src = NVLINK_DATASHEET_GBS, "H100 SXM data sheet (NVLink 4, per direction)"
     if a.peer_copy:
         g = peer_copy_gbs(w, dev)
+        if g:                                     # rank 0 of a multi-GPU run measures it
+            link_gbs, link_src = g, "peer copy measured in this run"
         if w.rank == 0:
             rows.append({"peer_copy_GBs": g, "bytes": 256 << 20, "how": "torch copy_ rank1 → rank0 over a VMM peer mapping, best of 5"})
             print(json.dumps(rows[-1]), flush=True)
@@ -180,9 +182,9 @@ def main():
             row = {"bytes": n * esz, "impl": impl, "n_gpus": w.size, "us": us, "tensors": len(shapes),
                    "gather_GBs": gather_b / us / 1e3 if w.size > 1 else None,
                    "bcast_GBs": bcast_b / us / 1e3,
-                   "roofline_us_770": need / (NVLINK_MEASURED_GBS * 1e3) if need else None,
-                   "roofline_frac_770": need / (NVLINK_MEASURED_GBS * 1e3) / us if need else None,
-                   "roofline_frac_900": need / (NVLINK_NOMINAL_GBS * 1e3) / us if need else None,
+                   "roofline_us": need / (link_gbs * 1e3) if need else None,
+                   "roofline_frac": need / (link_gbs * 1e3) / us if need else None,
+                   "roofline_GBs": link_gbs, "roofline_source": link_src,
                    "wire_bytes": wire, "dtype": a.dtype, "code": a.code,
                    "multicast": bool(eng is not None and eng.arena.has_multicast),
                    "reduce": {0: "p2p", 1: "multimem.ld_reduce"}.get(getattr(eng, "reduce", None)),

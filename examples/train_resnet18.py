@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""ResNet-18 synchronous parameter-server training on N B200s (BASELINE config 2), synthetic data.
+"""ResNet-18 synchronous parameter-server training on N H100s (BASELINE config 2), synthetic data.
 
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_resnet18.py
 """

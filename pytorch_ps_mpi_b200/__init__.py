@@ -1,4 +1,4 @@
-"""pytorch_ps_mpi_b200 — a Blackwell-native parameter-server data-parallel engine.
+"""pytorch_ps_mpi_b200 — a Hopper-native parameter-server data-parallel engine.
 
 Public surface of the reference (``/root/reference/__init__.py:1``: ``MPI_PS, Adam, SGD``) plus
 the coding plug-ins, the comm façade and the SPMD launcher.

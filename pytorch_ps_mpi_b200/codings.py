@@ -9,7 +9,7 @@ uses exactly three members of the object passed as ``code=``:
   decoding (``ps.py:165``).
 
 This module ships that contract as :class:`Coding` plus the built-ins the framework fuses into
-its sm_100a kernels: :class:`Identity`, :class:`Cast`, :class:`Scale`, :class:`TopK`.  Each
+its sm_90a kernels: :class:`Identity`, :class:`Cast`, :class:`Scale`, :class:`TopK`.  Each
 built-in has
 
 * a pure-PyTorch ``encode``/``decode`` (host slow path **and** the numerical oracle every CUDA

@@ -97,7 +97,7 @@ struct UpdatePlan {
     a.param_hyper = reinterpret_cast<const float2*>(param_hyper);
     a.timeout_ns = (unsigned long long)(timeout_s * 1e9);
     // Window the chunk: one launch touches at most `window_bytes` of every rank's wire arena.  A single kernel that walks
-    // >= 1 GB of mapped peer memory on each of 8 ranks falls off a TLB cliff (194 GB/s, profiles/bw_sweep_n8.json);
+    // >= 1 GB of mapped peer memory on each of 8 ranks falls off a TLB cliff;
     // back-to-back launches over <= 128 MB windows do not.  Only the first window waits for the flags (the rest is
     // stream-ordered behind it) and only the last one raises PARAMS_READY / CONSUMED / ACK.
     const int64_t per_tile = std::max<int64_t>(a.bytes_per_tile, 1);
@@ -200,7 +200,7 @@ void select_ready(uint64_t signal_local, uint64_t consumed, uint32_t cand_mask, 
 
 void snapshot(uint64_t signal_local, uint64_t stage, uint64_t shadow, uint64_t params, uint64_t nbytes, uint64_t scratch,
               int attempts, uint64_t stream) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   psb_launch_snapshot(pick_stream(stream), reinterpret_cast<const uint64_t*>(signal_local), reinterpret_cast<const void*>(stage),
@@ -214,7 +214,7 @@ void snapshot(uint64_t signal_local, uint64_t stage, uint64_t shadow, uint64_t p
 void bind_gemm(py::module_& m);   // gemm_bindings.cpp
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "pytorch_ps_mpi_b200 CUDA runtime: VMM symmetric memory + sm_100a kernels";
+  m.doc() = "pytorch_ps_mpi_b200 CUDA runtime: VMM symmetric memory + sm_90a kernels";
   m.attr("TILE") = PSB_TILE;
   m.attr("SIGNAL_SLOTS") = PSB_SIGNAL_SLOTS;
   m.attr("SIG_GRAD_READY") = SIG_GRAD_READY;

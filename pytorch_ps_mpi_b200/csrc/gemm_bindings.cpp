@@ -1,4 +1,4 @@
-// Bindings of the broadcast-gated tcgen05 GEMM (csrc/kernels/bcast_gemm.cu): builds the TMA
+// Bindings of the broadcast-gated wgmma GEMM (csrc/kernels/bcast_gemm.cu): builds the TMA
 // tensor maps with cuTensorMapEncodeTiled (resolved through the runtime, no -lcuda) and launches.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAStream.h>
@@ -52,22 +52,27 @@ at::Tensor bcast_gemm(const at::Tensor& x, uint64_t w_ptr, int64_t N, int64_t K,
   const int64_t M = x.size(0);
   auto y = at::empty({M, N}, x.options());
   if (M == 0) return y;
-  // cta_group::2 (two SMs per 256x256 tile) whenever there are at least 256 rows; `variant & 15` forces 1-CTA (1) / 2-CTA (2).
-  // bits 4-7: epilogue of the 2-CTA kernel — 0 auto (TMA store when N % 8 == 0, else staged), 1 staged, 3 TMA store,
-  // 4 the round-1 row-strided stores (bench/gemm_variants.py)
+  // a pair of CTAs (one cluster, the B tile multicast to both) whenever there are at least 256 rows; `variant & 15` forces
+  // one CTA (1) / a pair (2).  Bits 4-7: epilogue — 0 auto (TMA store when N % 8 == 0, else staged), 1 staged, 3 TMA store,
+  // 4 direct stores from the accumulator fragment (bench/gemm_variants.py)
   const int base = variant & 15, epi_sel = (variant >> 4) & 15;
   TORCH_CHECK(base <= 2 && (epi_sel == 0 || epi_sel == 1 || epi_sel == 3 || epi_sel == 4) && (variant >> 8) == 0,
               "unknown bcast_gemm variant ", variant);
-  TORCH_CHECK(epi_sel == 0 || base == 2, "epilogue variants need the 2-CTA kernel (variant & 15 == 2)");
   const int epi = epi_sel == 0 ? -1 : (epi_sel == 4 ? 0 : epi_sel);
+  TORCH_CHECK(epi != 3 || N % 8 == 0, "the TMA-store epilogue needs N % 8 == 0 (16-byte row pitch)");
   const bool two_cta = base == 2 || (base == 0 && M >= 256);
   CUtensorMap ma = make_map(reinterpret_cast<uint64_t>(x.data_ptr()), M, K, K, 128);
-  const int bnt2 = N <= 64 ? 64 : (N <= 128 ? 128 : 256);          // must match psb_launch_bcast_gemm's choice
-  CUtensorMap mb = make_map(w_ptr, N, K, K, two_cta ? bnt2 / 2 : 256);   // B box: half tile per CTA (2-CTA) or BN rows
+  const int bn = psb_bcast_gemm_bn((int)N);
+  CUtensorMap mb = make_map(w_ptr, N, K, K, two_cta ? bn / 2 : bn);   // B box: half tile per CTA of a pair, or the whole tile
+  CUtensorMap mc;
   BcastGemmArgs a{};
   a.tmap_a = &ma;
   a.tmap_b = &mb;
   a.tmap_c = y.data_ptr();
+  if (N % 8 == 0 && (epi == 3 || epi < 0)) {
+    mc = make_map(reinterpret_cast<uint64_t>(y.data_ptr()), M, N, N, 32);      // box: 64 columns x 32 rows, 128B swizzle
+    a.tmap_out = &mc;
+  }
   const float* bp = nullptr;
   at::Tensor bias_f;
   if (bias.has_value() && bias->defined()) {
@@ -82,19 +87,7 @@ at::Tensor bcast_gemm(const at::Tensor& x, uint64_t w_ptr, int64_t N, int64_t K,
   a.two_cta = two_cta ? 1 : 0;
   a.timeout_ns = (unsigned long long)(timeout_s * 1e9);
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
-  const cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-  if (two_cta) {
-    CUtensorMap mc;
-    const void* mcp = nullptr;
-    TORCH_CHECK(epi != 3 || N % 8 == 0, "the TMA-store epilogue needs N % 8 == 0 (16-byte row pitch)");
-    if (N % 8 == 0 && (epi == 3 || epi < 0)) {
-      mc = make_map(reinterpret_cast<uint64_t>(y.data_ptr()), M, N, N, 32);      // box: 64 columns x 32 rows, 128B swizzle
-      mcp = &mc;
-    }
-    psb_launch_bcast_gemm2(stream, a, sms, epi, mcp);
-  } else {
-    psb_launch_bcast_gemm(stream, a, sms);
-  }
+  psb_launch_bcast_gemm(c10::cuda::getCurrentCUDAStream().stream(), a, sms, epi);
   cudaError_t e = cudaGetLastError();
   TORCH_CHECK(e == cudaSuccess, "psb_bcast_gemm_kernel launch: ", cudaGetErrorString(e));
   return y;
@@ -122,19 +115,20 @@ std::vector<at::Tensor> bn_forward(const at::Tensor& x, c10::optional<at::Tensor
   TORCH_CHECK(running_mean.scalar_type() == at::kFloat && running_var.scalar_type() == at::kFloat, "running stats must be fp32");
   auto y = at::empty_like(x);
   auto fo = x.options().dtype(at::kFloat);
-  auto scratch = at::empty({6 * C}, fo);   // sums[2C] | mean | rstd | scale | shift
+  auto scratch = at::empty({4 * C}, fo);   // mean | rstd | scale | shift
   float* sp = scratch.data_ptr<float>();
-  at::Tensor mean = scratch.narrow(0, 2 * C, C), rstd = scratch.narrow(0, 3 * C, C);
+  at::Tensor mean = scratch.narrow(0, 0, C), rstd = scratch.narrow(0, C, C);
+  at::Tensor part = training ? at::empty({psb_bn_partial_floats(pixels, C)}, fo) : at::Tensor();
   // ReLU + training: a 1-bit-per-element mask (y > 0) for the backward, which then never re-reads y
   at::Tensor mask = (relu && training) ? at::empty({pixels * (C / 8)}, x.options().dtype(at::kByte)) : at::Tensor();
   if (!training) {   // inference: scale/shift from the running statistics
     auto r = (running_var + eps).rsqrt();
     auto sc = gamma.to(at::kFloat) * r;
-    scratch.narrow(0, 4 * C, C).copy_(sc);
-    scratch.narrow(0, 5 * C, C).copy_(beta.to(at::kFloat) - running_mean * sc);
+    scratch.narrow(0, 2 * C, C).copy_(sc);
+    scratch.narrow(0, 3 * C, C).copy_(beta.to(at::kFloat) - running_mean * sc);
   }
   psb_bn_forward(c10::cuda::getCurrentCUDAStream().stream(), x.data_ptr(), rp, gamma.data_ptr(), beta.data_ptr(), y.data_ptr(),
-                 sp, sp + 2 * C, sp + 3 * C, sp + 4 * C, sp + 5 * C, running_mean.data_ptr<float>(),
+                 part.defined() ? part.data_ptr<float>() : nullptr, sp, sp + C, sp + 2 * C, sp + 3 * C, running_mean.data_ptr<float>(),
                  running_var.data_ptr<float>(), pixels, C, (float)eps, (float)momentum, relu ? 1 : 0, training ? 1 : 0,
                  mask.defined() ? mask.data_ptr() : nullptr);
   cudaError_t e = cudaGetLastError();
@@ -167,11 +161,12 @@ std::vector<at::Tensor> bn_backward(const at::Tensor& dy, const at::Tensor& x, c
     return at::empty_like(gamma);
   };
   auto dgamma = pick(out_dgamma), dbeta = pick(out_dbeta);
-  auto scratch = at::empty({5 * C}, x.options().dtype(at::kFloat));
+  auto scratch = at::empty({3 * C}, x.options().dtype(at::kFloat));
+  auto part = at::empty({psb_bn_partial_floats(pixels, C)}, x.options().dtype(at::kFloat));
   float* sp = scratch.data_ptr<float>();
   psb_bn_backward(c10::cuda::getCurrentCUDAStream().stream(), dy.data_ptr(), x.data_ptr(),
-                  (relu && !masked) ? y.data_ptr() : nullptr, gamma.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), sp,
-                  sp + 2 * C, dx.data_ptr(), has_res ? dres.data_ptr() : nullptr, dgamma.data_ptr(), dbeta.data_ptr(), pixels, C,
+                  (relu && !masked) ? y.data_ptr() : nullptr, gamma.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
+                  part.data_ptr<float>(), sp, dx.data_ptr(), has_res ? dres.data_ptr() : nullptr, dgamma.data_ptr(), dbeta.data_ptr(), pixels, C,
                   relu ? 1 : 0, masked ? y.data_ptr() : nullptr);
   cudaError_t e = cudaGetLastError();
   TORCH_CHECK(e == cudaSuccess, "psb_bn_backward: ", cudaGetErrorString(e));
@@ -264,12 +259,13 @@ std::vector<at::Tensor> stem_fwd(const at::Tensor& x, const at::Tensor& w2d, boo
               "operands must be 16-byte aligned");
   const int OH = (H - 1) / 2 + 1, OW = (W - 1) / 2 + 1;
   auto y = at::empty({N, OH, OW, 64}, x.options());
-  at::Tensor sums = want_sums ? at::zeros({128}, x.options().dtype(at::kFloat)) : at::Tensor();
+  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  at::Tensor sums = want_sums ? at::empty({128}, x.options().dtype(at::kFloat)) : at::Tensor();
+  at::Tensor part = want_sums ? at::empty({sms, 128}, x.options().dtype(at::kFloat)) : at::Tensor();
   CUtensorMap mw = make_map(reinterpret_cast<uint64_t>(w2d.data_ptr()), 64, 176, 176, 64);
   CUtensorMap my = make_map(reinterpret_cast<uint64_t>(y.data_ptr()), (int64_t)N * OH * OW, 64, 64, OW);
-  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   psb_stem_fwd_launch(c10::cuda::getCurrentCUDAStream().stream(), &mw, &my, x.data_ptr(), want_sums ? sums.data_ptr<float>() : nullptr,
-                      N, H, W, sms, reinterpret_cast<const uint64_t*>(flag_ptr), epoch, (unsigned long long)(timeout_s * 1e9));
+                      want_sums ? part.data_ptr<float>() : nullptr, N, H, W, sms, reinterpret_cast<const uint64_t*>(flag_ptr), epoch, (unsigned long long)(timeout_s * 1e9));
   cudaError_t e = cudaGetLastError();
   TORCH_CHECK(e == cudaSuccess, "psb_stem_fwd_kernel launch: ", cudaGetErrorString(e));
   return {y.permute({0, 3, 1, 2}), sums};
@@ -356,7 +352,7 @@ void bind_gemm(py::module_& m) {
   m.def("bn_forward_presummed", &bn_forward_presummed, "BN forward with sums produced by the fused stem kernel");
   m.def("stem_fwd", &stem_fwd, py::arg("x"), py::arg("w2d"), py::arg("want_sums") = true, py::arg("flag_ptr") = 0,
         py::arg("epoch") = 0, py::arg("timeout_s") = 30.0,
-        "fused implicit-GEMM ResNet stem (+ BN statistics) on tcgen05; flag_ptr/epoch: PARAMS_READY gate of the weight load");
+        "fused implicit-GEMM ResNet stem (+ BN statistics) on wgmma; flag_ptr/epoch: PARAMS_READY gate of the weight load");
   m.def("stem_wgrad_finalize", &stem_wgrad_finalize, py::arg("partial"), py::arg("out") = c10::nullopt,
         "sum the per-CTA partials → dW2d [64,176] bf16 (optionally straight into the PS wire arena)");
   m.def("stem_wgrad", &stem_wgrad, "implicit weight gradient of the stem → per-CTA fp32 partials [grid,176,64]");
@@ -365,6 +361,6 @@ void bind_gemm(py::module_& m) {
         "fused channels-last bf16 BatchNorm(+residual)(+ReLU) backward");
   m.def("bcast_gemm", &bcast_gemm, py::arg("x"), py::arg("w_ptr"), py::arg("N"), py::arg("K"), py::arg("bias"),
         py::arg("relu"), py::arg("flag_ptr") = 0, py::arg("epoch") = 0, py::arg("timeout_s") = 30.0, py::arg("variant") = 0,
-        "tcgen05/TMEM/TMA GEMM whose weight tiles are gated on the PS broadcast epoch flag");
+        "wgmma/TMA GEMM whose weight tiles are gated on the PS broadcast epoch flag");
   m.def("bcast_gemm_smem_bytes", &psb_bcast_gemm_smem_bytes);
 }

@@ -1,8 +1,7 @@
-// Fused training BatchNorm for channels-last (NHWC) bf16 activations on sm_100a.
+// Fused training BatchNorm for channels-last (NHWC) bf16 activations on sm_90a.
 //
-// Why it exists: the launch list of one ResNet-18 step (profiles/resnet18_step_launches_n1.txt)
-// shows ATen's channels-last BatchNorm + the separate add / ReLU kernels taking ~45 % of the step
-// at ~0.5 TB/s.  BatchNorm is pure HBM traffic, so the framework ships its own:
+// Why it exists: ATen's channels-last BatchNorm + the separate add / ReLU kernels are a large share of a
+// ResNet-18 step and make 5-6 HBM passes.  BatchNorm is pure HBM traffic, so the framework ships its own:
 //   forward : psb_bn_stats   (1 read of x, fp32 sum / sum-of-squares per channel)
 //             psb_bn_finalize (C threads: mean, rstd, running stats, fused scale/shift)
 //             psb_bn_apply   (read x [+ residual] → y = act(x*scale + shift [+ residual]), 1 write)
@@ -39,10 +38,10 @@ __device__ __forceinline__ void st8(__nv_bfloat16* p, const float* f) {
                                              pack_bf16x2(f[6], f[7]));
 }
 
-// Block-level reduction of per-thread 8-channel partials over the pixel lanes, then one atomicAdd
-// per channel per CTA.  smem layout: [lanes][C] floats.
-__device__ __forceinline__ void reduce_lanes_atomic(float* smem, const float* part, int tx, int ty, const BnGeom& g,
-                                                    float* out) {
+// Block-level reduction of per-thread 8-channel partials over the pixel lanes, then one plain store per channel into this
+// CTA's row of the partials (no atomics: the finalize kernels add the rows in CTA order, so every run sums in the same order
+// and gets the same bits).  smem layout: [lanes][C] floats.
+__device__ __forceinline__ void reduce_lanes(float* smem, const float* part, int tx, int ty, const BnGeom& g, float* out) {
   if (ty < g.lanes) {   // threads beyond lanes*groups (C/8 not dividing 256) hold no partials
     float4* row = reinterpret_cast<float4*>(smem + (size_t)ty * g.C + tx * 8);
     row[0] = make_float4(part[0], part[1], part[2], part[3]);
@@ -52,13 +51,13 @@ __device__ __forceinline__ void reduce_lanes_atomic(float* smem, const float* pa
   for (int c = threadIdx.x; c < g.C; c += BN_THREADS) {
     float s = 0.f;
     for (int l = 0; l < g.lanes; ++l) s += smem[(size_t)l * g.C + c];
-    atomicAdd(out + c, s);
+    out[c] = s;
   }
   __syncthreads();
 }
 
 // ---- forward ------------------------------------------------------------------------------
-__global__ void __launch_bounds__(BN_THREADS) psb_bn_stats(const __nv_bfloat16* __restrict__ x, float* __restrict__ sums,
+__global__ void __launch_bounds__(BN_THREADS) psb_bn_stats(const __nv_bfloat16* __restrict__ x, float* __restrict__ part,
                                                             BnGeom g) {
   extern __shared__ float smem[];
   const int tx = threadIdx.x % g.groups, ty = threadIdx.x / g.groups;
@@ -92,20 +91,45 @@ __global__ void __launch_bounds__(BN_THREADS) psb_bn_stats(const __nv_bfloat16* 
       }
     }
   }
-  reduce_lanes_atomic(smem, s, tx, ty, g, sums);
-  reduce_lanes_atomic(smem, q, tx, ty, g, sums + g.C);
+  reduce_lanes(smem, s, tx, ty, g, part + (size_t)blockIdx.x * 2 * g.C);
+  reduce_lanes(smem, q, tx, ty, g, part + (size_t)blockIdx.x * 2 * g.C + g.C);
 }
 
-// sums[0:C]=Σx, sums[C:2C]=Σx² → mean/rstd (saved for backward), running stats, fused scale/shift
-__global__ void psb_bn_finalize(const float* __restrict__ sums, const __nv_bfloat16* __restrict__ gamma,
-                                const __nv_bfloat16* __restrict__ beta, float* __restrict__ mean, float* __restrict__ rstd,
-                                float* __restrict__ scale, float* __restrict__ shift, float* running_mean,
-                                float* running_var, int C, long long pixels, float eps, float momentum) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
+// Σ over `nparts` rows of per-CTA partials [nparts][2C] for the block's FIN_CH channels, in a fixed order: slice i adds rows
+// i, i + FIN_SLICES, ... and thread 0 of each channel adds the slices in order.  Returns false on threads that hold no result.
+constexpr int FIN_CH = 32, FIN_SLICES = 8, FIN_THREADS = FIN_CH * FIN_SLICES;
+__device__ __forceinline__ bool sum_partials(const float* __restrict__ part, int nparts, int C, float& s, float& q, int& c) {
+  __shared__ float red[2][FIN_SLICES][FIN_CH];
+  const int cl = threadIdx.x % FIN_CH, sl = threadIdx.x / FIN_CH;
+  c = blockIdx.x * FIN_CH + cl;
+  s = 0.f, q = 0.f;
+  if (c < C)
+    for (int b = sl; b < nparts; b += FIN_SLICES) {
+      s += part[(size_t)b * 2 * C + c];
+      q += part[(size_t)b * 2 * C + C + c];
+    }
+  red[0][sl][cl] = s;
+  red[1][sl][cl] = q;
+  __syncthreads();
+  if (sl != 0 || c >= C) return false;
+  s = 0.f, q = 0.f;
+  for (int i = 0; i < FIN_SLICES; ++i) s += red[0][i][cl], q += red[1][i][cl];
+  return true;
+}
+
+// partials of Σx | Σx² → mean/rstd (saved for backward), running stats, fused scale/shift
+__global__ void __launch_bounds__(FIN_THREADS) psb_bn_finalize(const float* __restrict__ part, int nparts,
+                                                                const __nv_bfloat16* __restrict__ gamma,
+                                                                const __nv_bfloat16* __restrict__ beta, float* __restrict__ mean,
+                                                                float* __restrict__ rstd, float* __restrict__ scale,
+                                                                float* __restrict__ shift, float* running_mean, float* running_var,
+                                                                int C, long long pixels, float eps, float momentum) {
+  float sx, sxx;
+  int c;
+  if (!sum_partials(part, nparts, C, sx, sxx, c)) return;
   const float inv_n = 1.f / (float)pixels;
-  const float m = sums[c] * inv_n;
-  float var = fmaf(-m, m, sums[C + c] * inv_n);
+  const float m = sx * inv_n;
+  float var = fmaf(-m, m, sxx * inv_n);
   var = fmaxf(var, 0.f);
   const float r = rsqrtf(var + eps);
   mean[c] = m;
@@ -178,7 +202,7 @@ __global__ void __launch_bounds__(BN_THREADS) psb_bn_bwd_reduce(const __nv_bfloa
                                                                  const __nv_bfloat16* __restrict__ y,
                                                                  const uint8_t* __restrict__ mask,
                                                                  const float* __restrict__ mean, const float* __restrict__ rstd,
-                                                                 float* __restrict__ sums, BnGeom g) {
+                                                                 float* __restrict__ part, BnGeom g) {
   extern __shared__ float smem[];
   const int tx = threadIdx.x % g.groups, ty = threadIdx.x / g.groups;
   float s[8], q[8], mu[8], rs[8];
@@ -227,19 +251,21 @@ __global__ void __launch_bounds__(BN_THREADS) psb_bn_bwd_reduce(const __nv_bfloa
       }
     }
   }
-  reduce_lanes_atomic(smem, s, tx, ty, g, sums);
-  reduce_lanes_atomic(smem, q, tx, ty, g, sums + g.C);
+  reduce_lanes(smem, s, tx, ty, g, part + (size_t)blockIdx.x * 2 * g.C);
+  reduce_lanes(smem, q, tx, ty, g, part + (size_t)blockIdx.x * 2 * g.C + g.C);
 }
 
 // dx = gamma*rstd * (dy' - mean(dy') - x̂ * mean(dy'·x̂))  =  dy'*a + x*b + c   per channel
-__global__ void psb_bn_bwd_finalize(const float* __restrict__ sums, const __nv_bfloat16* __restrict__ gamma,
-                                    const float* __restrict__ mean, const float* __restrict__ rstd, float* __restrict__ ca,
-                                    float* __restrict__ cb, float* __restrict__ cc, __nv_bfloat16* __restrict__ dgamma,
-                                    __nv_bfloat16* __restrict__ dbeta, int C, long long pixels) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
+__global__ void __launch_bounds__(FIN_THREADS) psb_bn_bwd_finalize(const float* __restrict__ part, int nparts,
+                                                                    const __nv_bfloat16* __restrict__ gamma,
+                                                                    const float* __restrict__ mean, const float* __restrict__ rstd,
+                                                                    float* __restrict__ ca, float* __restrict__ cb,
+                                                                    float* __restrict__ cc, __nv_bfloat16* __restrict__ dgamma,
+                                                                    __nv_bfloat16* __restrict__ dbeta, int C, long long pixels) {
+  float sdy, sdyx;
+  int c;
+  if (!sum_partials(part, nparts, C, sdy, sdyx, c)) return;
   const float inv_n = 1.f / (float)pixels;
-  const float sdy = sums[c], sdyx = sums[C + c];
   const float g = gamma ? __bfloat162float(gamma[c]) : 1.f;
   const float r = rstd[c], m = mean[c];
   const float a = g * r;
@@ -286,9 +312,8 @@ __global__ void __launch_bounds__(BN_THREADS) psb_bn_bwd_apply(const __nv_bfloat
 }
 
 // (A fused BatchNorm-apply + ReLU + 3x3/s2 max-pool pair lived here in round 2: per-pixel gather, then a 2x2-quad backward.
-//  It was correct but never beat the unfused kernels once those got the 1-bit ReLU mask and the quad max-pool backward —
-//  forward 0.39 vs 0.49 ms, forward+backward 1.31 vs 1.19 ms at batch 256 — and was deleted; the measurements are in
-//  profiles/bnpool_fusion_REJECTED.jsonl.)
+//  It was correct but never beat the unfused kernels once those got the 1-bit ReLU mask and the quad max-pool backward,
+//  and was deleted.)
 BnGeom geom(long long pixels, int C) {
   BnGeom g;
   g.pixels = pixels;
@@ -300,23 +325,27 @@ BnGeom geom(long long pixels, int C) {
 }
 
 int grid_for(long long pixels, const BnGeom& g, int min_iters = 1) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long want = (pixels + (long long)g.lanes * min_iters - 1) / ((long long)g.lanes * min_iters);   // >= min_iters pixel batches per CTA
   long long cap = (long long)sms * 8;
   return (int)(want < cap ? (want > 0 ? want : 1) : cap);
 }
-// The reducing kernels end with 2C float atomics per CTA: on the small late-stage tensors (12 544 pixels x 512 channels) 1 184
-// CTAs of ~3 pixel batches each spent their time in 1.2 M contended atomics — every statistics / backward-reduce launch had
-// a ~16 us floor whatever its size (profiles/resnet18_step_launches_r2.txt).  They get at least 8 batches per CTA.
+// The reducing kernels write 2C partials per CTA that the finalize kernels add up: on the small late-stage tensors thousands of
+// CTAs of ~3 pixel batches each would make that sum the bottleneck.  They get at least 8 batches per CTA.
 constexpr int REDUCE_MIN_ITERS = 8;
 
 }  // namespace
 
+// floats of per-CTA partials the reducing kernels write for a tensor of `pixels` x C (the `part` argument below)
+long long psb_bn_partial_floats(long long pixels, int C) {
+  return (long long)grid_for(pixels, geom(pixels, C), REDUCE_MIN_ITERS) * 2 * C;
+}
+
 // C must be a multiple of 8 and <= 2048 (groups <= 256)
 void psb_bn_forward(cudaStream_t s, const void* x, const void* res, const void* gamma, const void* beta, void* y,
-                    float* sums /*2C, zeroed here*/, float* mean, float* rstd, float* scale, float* shift, float* running_mean,
+                    float* part /*psb_bn_partial_floats*/, float* mean, float* rstd, float* scale, float* shift, float* running_mean,
                     float* running_var, long long pixels, int C, float eps, float momentum, int relu, int training, void* mask) {
   auto MK = reinterpret_cast<uint8_t*>(mask);
   const BnGeom g = geom(pixels, C);
@@ -326,9 +355,9 @@ void psb_bn_forward(cudaStream_t s, const void* x, const void* res, const void* 
   auto Y = reinterpret_cast<__nv_bfloat16*>(y);
   psb_count_launch(training ? 3 : 1);
   if (training) {
-    cudaMemsetAsync(sums, 0, sizeof(float) * 2 * C, s);
-    psb_bn_stats<<<grid_for(pixels, g, REDUCE_MIN_ITERS), BN_THREADS, sizeof(float) * g.lanes * C, s>>>(X, sums, g);
-    psb_bn_finalize<<<(C + 127) / 128, 128, 0, s>>>(sums, reinterpret_cast<const __nv_bfloat16*>(gamma),
+    const int rgrid = grid_for(pixels, g, REDUCE_MIN_ITERS);
+    psb_bn_stats<<<rgrid, BN_THREADS, sizeof(float) * g.lanes * C, s>>>(X, part, g);
+    psb_bn_finalize<<<(C + FIN_CH - 1) / FIN_CH, FIN_THREADS, 0, s>>>(part, rgrid, reinterpret_cast<const __nv_bfloat16*>(gamma),
                                                      reinterpret_cast<const __nv_bfloat16*>(beta), mean, rstd, scale, shift,
                                                      running_mean, running_var, C, pixels, eps, momentum);
   }
@@ -354,7 +383,7 @@ void psb_bn_forward_presummed(cudaStream_t s, const void* x, const void* res, co
   auto R = reinterpret_cast<const __nv_bfloat16*>(res);
   auto Y = reinterpret_cast<__nv_bfloat16*>(y);
   psb_count_launch(2);
-  psb_bn_finalize<<<(C + 127) / 128, 128, 0, s>>>(sums, reinterpret_cast<const __nv_bfloat16*>(gamma),
+  psb_bn_finalize<<<(C + FIN_CH - 1) / FIN_CH, FIN_THREADS, 0, s>>>(sums, 1, reinterpret_cast<const __nv_bfloat16*>(gamma),
                                                    reinterpret_cast<const __nv_bfloat16*>(beta), mean, rstd, scale, shift,
                                                    running_mean, running_var, C, pixels, eps, momentum);
   if (res != nullptr) {
@@ -367,7 +396,7 @@ void psb_bn_forward_presummed(cudaStream_t s, const void* x, const void* res, co
 }
 
 void psb_bn_backward(cudaStream_t s, const void* dy, const void* x, const void* y, const void* gamma, const float* mean,
-                     const float* rstd, float* sums /*2C*/, float* coef /*3C*/, void* dx, void* dres, void* dgamma, void* dbeta,
+                     const float* rstd, float* part /*psb_bn_partial_floats*/, float* coef /*3C*/, void* dx, void* dres, void* dgamma, void* dbeta,
                      long long pixels, int C, int relu, const void* mask) {
   auto MK = reinterpret_cast<const uint8_t*>(mask);
   const BnGeom g = geom(pixels, C);
@@ -376,13 +405,13 @@ void psb_bn_backward(cudaStream_t s, const void* dy, const void* x, const void* 
   auto X = reinterpret_cast<const __nv_bfloat16*>(x);
   auto Y = reinterpret_cast<const __nv_bfloat16*>(y);
   psb_count_launch(3);
-  cudaMemsetAsync(sums, 0, sizeof(float) * 2 * C, s);
   const size_t sm = sizeof(float) * g.lanes * C;
   const int rgrid = grid_for(pixels, g, REDUCE_MIN_ITERS);
-  if (relu && MK) psb_bn_bwd_reduce<true, true><<<rgrid, BN_THREADS, sm, s>>>(DY, X, Y, MK, mean, rstd, sums, g);
-  else if (relu) psb_bn_bwd_reduce<true, false><<<rgrid, BN_THREADS, sm, s>>>(DY, X, Y, MK, mean, rstd, sums, g);
-  else psb_bn_bwd_reduce<false, false><<<rgrid, BN_THREADS, sm, s>>>(DY, X, Y, MK, mean, rstd, sums, g);
-  psb_bn_bwd_finalize<<<(C + 127) / 128, 128, 0, s>>>(sums, reinterpret_cast<const __nv_bfloat16*>(gamma), mean, rstd, coef,
+  if (relu && MK) psb_bn_bwd_reduce<true, true><<<rgrid, BN_THREADS, sm, s>>>(DY, X, Y, MK, mean, rstd, part, g);
+  else if (relu) psb_bn_bwd_reduce<true, false><<<rgrid, BN_THREADS, sm, s>>>(DY, X, Y, MK, mean, rstd, part, g);
+  else psb_bn_bwd_reduce<false, false><<<rgrid, BN_THREADS, sm, s>>>(DY, X, Y, MK, mean, rstd, part, g);
+  psb_bn_bwd_finalize<<<(C + FIN_CH - 1) / FIN_CH, FIN_THREADS, 0, s>>>(part, rgrid, reinterpret_cast<const __nv_bfloat16*>(gamma),
+                                                                         mean, rstd, coef,
                                                        coef + C, coef + 2 * C, reinterpret_cast<__nv_bfloat16*>(dgamma),
                                                        reinterpret_cast<__nv_bfloat16*>(dbeta), C, pixels);
   auto DX = reinterpret_cast<__nv_bfloat16*>(dx);

@@ -1,4 +1,4 @@
-// Shared device helpers for the pytorch_ps_mpi_b200 sm_100a kernels.
+// Shared device helpers for the pytorch_ps_mpi_b200 sm_90a kernels.
 //
 // Layout contract (mirrors pytorch_ps_mpi_b200/codings.py and parallel/layout.py):
 //   * every parameter occupies an integral number of PSB_TILE-element tiles of one flat arena,

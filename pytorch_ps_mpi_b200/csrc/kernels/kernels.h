@@ -1,4 +1,4 @@
-// Host-callable launchers of the sm_100a kernels (plain C++ types; no torch headers here).
+// Host-callable launchers of the sm_90a kernels (plain C++ types; no torch headers here).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -98,7 +98,7 @@ void psb_launch_snapshot(cudaStream_t s, const uint64_t* signal_local, const voi
                          unsigned long long* scratch, int attempts, int num_sms);
 int psb_update_max_grid(int kind, int wire, int opt);
 
-// bcast_gemm.cu — tcgen05 / TMEM / TMA GEMM whose weight tiles are gated on the PS broadcast epoch
+// bcast_gemm.cu — wgmma / TMA GEMM whose weight tiles are gated on the PS broadcast epoch
 struct BcastGemmArgs {
   const void* tmap_a;   // CUtensorMap* (host memory, passed as __grid_constant__ by value in launcher)
   const void* tmap_b;
@@ -108,26 +108,28 @@ struct BcastGemmArgs {
   uint64_t ready_epoch;
   int32_t M, N, K;
   int32_t relu;
-  int32_t two_cta;      // 1 → cta_group::2 kernel (256x256 tiles per CTA pair; B box = 128 rows)
-  const void* tmap_out; // 2-CTA only: CUtensorMap* of the [M,N] output (box 64 x 32, 128B swizzle) for the TMA-store
-                        // epilogue; nullptr (or N % 8 != 0) → staged full-line stores
+  int32_t two_cta;      // 1 → clusters of two CTAs on 256-row tiles sharing (multicasting) the B tile; B box = BN/2 rows
+  const void* tmap_out; // CUtensorMap* of the [M,N] output (box 64 x 32, 128B swizzle) for the TMA-store epilogue;
+                        // nullptr (or N % 8 != 0) → staged full-line stores
   unsigned long long timeout_ns;
 };
-void psb_launch_bcast_gemm(cudaStream_t s, const BcastGemmArgs& a, int num_sms);
-// bcast_gemm2.cu — the cta_group::2 kernel; epi -1 = auto (TMA-store / staged epilogue), 0 / 1 / 3 = force (bench/gemm_variants.py)
-void psb_launch_bcast_gemm2(cudaStream_t s, const BcastGemmArgs& a, int num_sms, int epi, const void* tmap_out);
+// epi: -1 = auto (TMA store when N % 8 == 0 and tmap_out is given, else staged), 0 direct / 1 staged / 3 TMA store = force
+void psb_launch_bcast_gemm(cudaStream_t s, const BcastGemmArgs& a, int num_sms, int epi);
+int psb_bcast_gemm_bn(int N);   // the N extent of an output tile (the B box is this many rows, or half of it with two_cta)
 
 // bn_kernels.cu — fused channels-last bf16 BatchNorm (+residual, +ReLU), forward and backward
-void psb_bn_forward(cudaStream_t s, const void* x, const void* res, const void* gamma, const void* beta, void* y, float* sums,
+// `part`: per-CTA partial sums (psb_bn_partial_floats(pixels, C) floats), added in a fixed order: same inputs, same bits
+long long psb_bn_partial_floats(long long pixels, int C);
+void psb_bn_forward(cudaStream_t s, const void* x, const void* res, const void* gamma, const void* beta, void* y, float* part,
                     float* mean, float* rstd, float* scale, float* shift, float* running_mean, float* running_var,
                     long long pixels, int C, float eps, float momentum, int relu, int training,
                     void* mask = nullptr /* [pixels * C/8] bytes: 1 bit per element, y > 0 (relu + training) */);
 void psb_bn_forward_presummed(cudaStream_t s, const void* x, const void* res, const void* gamma, const void* beta, void* y,
-                              const float* sums, float* mean, float* rstd, float* scale, float* shift, float* running_mean,
+                              const float* sums /*2C*/, float* mean, float* rstd, float* scale, float* shift, float* running_mean,
                               float* running_var, long long pixels, int C, float eps, float momentum, int relu,
                               void* mask = nullptr);
 void psb_bn_backward(cudaStream_t s, const void* dy, const void* x, const void* y, const void* gamma, const float* mean,
-                     const float* rstd, float* sums, float* coef, void* dx, void* dres, void* dgamma, void* dbeta,
+                     const float* rstd, float* part, float* coef, void* dx, void* dres, void* dgamma, void* dbeta,
                      long long pixels, int C, int relu, const void* mask = nullptr /* the forward's ReLU bit mask, replaces y */);
 
 // pool_kernels.cu — channels-last bf16 3x3/s2/p1 max pooling
@@ -139,7 +141,8 @@ void psb_normalize_nhwc3_launch(cudaStream_t s, const void* x, void* y, const fl
 
 // stem_kernels.cu — fused implicit-GEMM ResNet stem (7x7/s2, 3 → 64) with BN statistics in the epilogue
 int psb_stem_fwd_smem_bytes();
-void psb_stem_fwd_launch(cudaStream_t s, const void* tmap_w, const void* tmap_y, const void* x, float* sums, int N, int H, int W,
+void psb_stem_fwd_launch(cudaStream_t s, const void* tmap_w, const void* tmap_y, const void* x, float* sums, float* part, int N,
+                         int H, int W,
                          int num_sms, const uint64_t* ready_flag, uint64_t ready_epoch, unsigned long long timeout_ns);
 
 int psb_stem_wgrad_grid(int N, int H, int num_sms);

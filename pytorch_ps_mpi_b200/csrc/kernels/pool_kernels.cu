@@ -1,6 +1,5 @@
 // 3x3 / stride-2 / pad-1 max pooling for channels-last bf16 activations, forward + backward.
-// ATen's max_pool_{forward,backward}_nhwc take 0.76 ms + 1.73 ms of a ResNet-18 step on B200
-// (profiles/resnet18_step_launches_n1.txt) for ~0.6 GB of traffic; these move 16 bytes per thread,
+// ATen's max_pool_{forward,backward}_nhwc are slow for the ~0.6 GB of traffic of a ResNet-18 step; these move 16 bytes per thread,
 // keep a 1-byte window position per output element for the backward, and the backward GATHERS
 // (each input pixel looks at the <= 4 windows covering it) so it needs no atomics and writes dx once.
 #include <cuda_bf16.h>
@@ -99,10 +98,10 @@ __global__ void __launch_bounds__(256) psb_maxpool_bwd(const __nv_bfloat16* __re
 }
 
 // ---- row-based variants (round 2) -----------------------------------------------------------------------------------
-// The kernels above spend most of their instructions on 64-bit div/mod index chains (one per 16 bytes) and ran at 2.7 / 1.6
-// TB/s (profiles/resnet18_step_launches_r2.txt: 207 + 350 us for 565 MB each).  Here a CTA walks whole rows with 32-bit
+// The kernels above spend most of their instructions on 64-bit div/mod index chains (one per 16 bytes).  Here a CTA walks whole rows with 32-bit
 // indices; tx = channel group of 8, ty = pixel lane, so a warp covers 32 / groups consecutive NHWC pixels.
-__global__ void __launch_bounds__(256) psb_maxpool_fwd_rows(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
+// (min-blocks 1: ptxas for sm_90a otherwise caps it at 40 registers and spills; it takes 48 without the cap)
+__global__ void __launch_bounds__(256, 1) psb_maxpool_fwd_rows(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                                             uint8_t* __restrict__ arg, PoolGeom g, int lanes) {
   const int tx = threadIdx.x % g.groups, ty = threadIdx.x / g.groups;
   if (ty >= lanes) return;
@@ -198,7 +197,7 @@ __global__ void __launch_bounds__(256) psb_maxpool_bwd_quads(const __nv_bfloat16
 }
 
 int pool_grid(long long total) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long want = (total + 255) / 256;
@@ -241,7 +240,7 @@ void psb_maxpool3x3s2_backward(cudaStream_t s, const void* dy, const void* arg, 
 // ---- input pre-processing: uint8 NCHW image → normalised bf16 NHWC padded to 8 channels --------------
 // One pass instead of ATen's float() / sub / div / to(bf16) / contiguous(channels_last) chain, and the
 // 8-channel (16-byte) pixel lets cuDNN run the 7x7 stem convolution on its aligned tensor-core kernels
-// (the 3-channel stem was 23 % of the step: profiles/resnet18_step_launches_fused.txt).
+// (C=3 defeats them).
 namespace {
 __global__ void __launch_bounds__(256) psb_normalize_pad8(const uint8_t* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                                           float m0, float m1, float m2, float s0, float s1, float s2, int N,
@@ -263,15 +262,14 @@ void psb_normalize_pad8_launch(cudaStream_t s, const void* x, void* y, const flo
                                                       mean[0], mean[1], mean[2], inv_std[0], inv_std[1], inv_std[2], N, HW);
 }
 
-// ---- ResNet stem as an implicit GEMM on OUR tcgen05 kernel ----------------------------------------------
-// cuDNN's 7x7/stride-2 convolution with 3 input channels takes 1.5 ms (fprop) + 1.0 ms (wgrad) of the
-// 10.5 ms ResNet-18 step on B200 (23 %, sm80-era kernels: C=3 defeats its tensor-core paths, and padding
-// C to 4/8 is slower still — scratch/stem_bench.py).  We lower it ourselves: psb_im2col_stem writes the
+// ---- ResNet stem as an implicit GEMM on OUR wgmma kernel -----------------------------------------------
+// cuDNN's 7x7/stride-2 convolution with 3 input channels cannot use its tensor-core paths (C=3).  We lower it
+// ourselves: psb_im2col_stem writes the
 // [N*OH*OW, 176] patch matrix (7 kernel rows x (21 real + 3 zero) columns + 8 zero columns), the forward
-// is psb_bcast_gemm (tcgen05/TMEM/TMA) against the matching [64,176] weight matrix and lands
+// is psb_bcast_gemm (wgmma/TMA) against the matching [64,176] weight matrix and lands
 // directly in NHWC, and the weight gradient is one library GEMM dY^T · A.
 namespace {
-constexpr int STEM_K = 176;   // 7 kernel rows x 24 (21 = 7*3 real + 3 zero, so every row starts 16-byte aligned) + 8 pad → 11 * UMMA_K
+constexpr int STEM_K = 176;   // 7 kernel rows x 24 (21 = 7*3 real + 3 zero, so every row starts 16-byte aligned) + 8 pad → 11 wgmma K steps
 
 // One thread = one (output pixel, kernel row): the 21 input values x[n, ih, iw0..iw0+6, 0..2] are CONTIGUOUS
 // in NHWC memory (42 bytes, always 2-mod-4 aligned because iw0 = 2*ow - 3 is odd), so they are fetched with

@@ -1,4 +1,4 @@
-// Parameter-server hot path for sm_100a: gradient encode, fused gather-reduce-decode-update-
+// Parameter-server hot path for sm_90a: gradient encode, fused gather-reduce-decode-update-
 // broadcast, and the epoch-flag signalling kernels.
 //
 // What these replace in the reference (citations into /root/reference):
@@ -808,8 +808,8 @@ __global__ void __launch_bounds__(256) psb_snapshot_commit(const __grid_constant
 
 template <int KIND, int WIRE, int OPT>
 void launch_update_t(cudaStream_t s, const UpdateArgs& a, int grid) {
-  // (a variant with two P2P tiles in flight per thread and no state prefetch measured slower, 72.6 us vs 52.5 us on the
-  //  ResNet-18 arena at N = 1, and was removed: profiles/psb_update_kernel_resnet18_n1_v2.ncu.txt)
+  // (a variant with two P2P tiles in flight per thread and no state prefetch measured slower on the ResNet-18 arena at
+  //  N = 1, and was removed)
   psb_update_kernel<KIND, WIRE, OPT><<<grid, PSB_THREADS, 0, s>>>(a);
 }
 template <int KIND, int WIRE>
@@ -865,7 +865,7 @@ void psb_launch_update(cudaStream_t s, int kind, int wire, int opt, const Update
 }
 
 int psb_update_max_grid(int kind, int wire, int opt) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   (void)kind, (void)wire, (void)opt;

@@ -1,29 +1,24 @@
-// The ResNet stem (default path since round 2; PSB200_STEM=im2col falls back) — 7x7 / stride 2 / pad 3 convolution, 3 → 64 channels —
-// as ONE implicit-GEMM kernel on tcgen05, replacing psb_im2col_stem (writes a 1.13 GB patch matrix at batch 256) +
-// psb_bcast_gemm2_kernel (reads it back) + the BatchNorm statistics pass over the 411 MB output
-// (profiles/resnet18_step_launches_final.txt: 355 + 505 + ~95 us of a 7.9 ms step).
+// The ResNet stem (default path; PSB200_STEM=im2col falls back) — 7x7 / stride 2 / pad 3 convolution, 3 → 64 channels — as
+// ONE implicit-GEMM kernel on wgmma, replacing psb_im2col_stem (writes a 1.13 GB patch matrix at batch 256) + the GEMM that
+// reads it back + the BatchNorm statistics pass over the 411 MB output.
 //
 // One tile = one output row (n, oh): OW <= 128 pixels x 64 channels, K = 176 (7 kernel rows x 24 columns — 21 real,
 // 3 zero — + 8 zero columns: the layout of ops/stem.py, so the same [64,176] weight matrix is used).
 //
-//   warps 0-3  builders   cp.async the 7 input rows of the NEXT tile into a zero-margined smem patch while building
-//                         the CURRENT tile's A operand: thread m copies, for each kernel row, the 42 contiguous
-//                         bytes x[n, 2oh-3+kh, 2m-3 .. 2m+3, 0..2] into the 128B-swizzled K-major UMMA layout
-//                         (three [128 x 64] bf16 blocks; the same canonical layout TMA would have produced)
-//   warp  8    MMA        11 x tcgen05.mma.cta_group::1.kind::f16 (128 x 64 x 16) per tile, accumulators
-//                         double-buffered in TMEM; the [64,176] weight operand is TMA-loaded once per CTA
-//   warps 4-7  epilogue   tcgen05.ld → bf16 → swizzled staging tile → ONE cp.async.bulk.tensor store per output row
-//                         (NHWC: the row is 14 KB contiguous), and the per-channel Σy / Σy² of the staged bf16 values
-//                         (exactly what psb_bn_stats would read back) accumulated in registers, 2 x 64 atomics per CTA
-//
-// Expected (desk estimate, to be measured): ~1000-1500 cycles per tile per SM → 0.15-0.25 ms for batch 256
-// versus ~0.95 ms for the three passes it replaces.
+//   warpgroup 0     builders   cp.async the 7 input rows of the NEXT tile into a zero-margined smem patch while building
+//                              the CURRENT tile's A operand: thread m copies, for each kernel row, the 42 contiguous
+//                              bytes x[n, 2oh-3+kh, 2m-3 .. 2m+3, 0..2] into the 128B-swizzled K-major wgmma layout
+//                              (three [128 x 64] bf16 blocks; the same canonical layout TMA would have produced)
+//   warpgroups 1-2  MMA +      64 pixel rows each: 11 x wgmma m64n64k16 per tile; the [64,176] weight operand is TMA-loaded
+//                   epilogue   once per CTA.  Then bf16 → swizzled staging tile → ONE cp.async.bulk.tensor store per output row
+//                              (NHWC: the row is 14 KB contiguous), and the per-channel Σy / Σy² of the staged bf16 values
+//                              (exactly what psb_bn_stats would read back) accumulated in registers, summed in CTA order
 #include "gemm_common.cuh"
 
 namespace {
 
 constexpr int SK = 176;                 // GEMM K (ops/stem.py STEM_K)
-constexpr int S_THREADS = 288;          // 4 builder + 4 epilogue + 1 MMA warp
+constexpr int S_THREADS = 384;          // builder + 2 MMA / epilogue warpgroups
 constexpr int SA_BLK = 128 * 128;       // one k-block of A: 128 rows x 128 B
 constexpr int SA_BYTES = 3 * SA_BLK;    // 48 KB per A buffer
 constexpr int SB_BLK = 64 * 128;        // one k-block of B (64 output channels)
@@ -44,7 +39,7 @@ static_assert(STEM_SMEM <= 232448, "shared memory budget");
 
 struct StemParams {
   const __nv_bfloat16* x;     // [N, H, W, 3] bf16 (channels-last, already normalised)
-  float* sums;                // [128]: Σy[64] | Σy²[64], accumulated with atomics (caller zeroes); nullable
+  float* sums;                // [gridDim.x][128]: this CTA's Σy[64] | Σy²[64] (summed in CTA order afterwards); nullable
   int N, H, W, OH, OW;
   // The broadcast gate (as in bcast_gemm*.cu): the weight matrix lives IN the symmetric parameter arena in the [64,176]
   // GEMM layout (layout.py custom placement) and the lane that TMA-loads it first acquires the PS's PARAMS_READY epoch, so
@@ -56,9 +51,6 @@ struct StemParams {
   unsigned long long timeout_ns;
 };
 
-__device__ __forceinline__ void named_bar(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
@@ -74,9 +66,6 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
   uint32_t v;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
   return v;
-}
-__host__ __device__ constexpr uint32_t stem_idesc() {   // D=f32, A=B=bf16, K-major, M=128, N=64
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
 }
 
 // queue the 7 input rows of output row `tile` into `patch` (cp.async; rows outside the image are zero-filled)
@@ -133,10 +122,7 @@ psb_stem_fwd_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_con
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* b_full = bars;            // [1]  weights landed
   uint64_t* a_full = bars + 1;        // [2]  4 builder warps arrive
-  uint64_t* a_empty = bars + 3;       // [2]  tcgen05.commit
-  uint64_t* t_full = bars + 5;        // [2]  tcgen05.commit (accumulator ready)
-  uint64_t* t_empty = bars + 7;       // [2]  4 epilogue warps arrive
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 9);
+  uint64_t* a_empty = bars + 3;       // [2]  the wgmmas of both MMA warpgroups that read A[buf] have retired
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles = p.N * p.OH;
@@ -152,9 +138,7 @@ psb_stem_fwd_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_con
     mbar_init(b_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&a_full[i], 4);
-      mbar_init(&a_empty[i], 1);
-      mbar_init(&t_full[i], 1);
-      mbar_init(&t_empty[i], 4);
+      mbar_init(&a_empty[i], 2);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -163,15 +147,6 @@ psb_stem_fwd_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_con
   for (int i = threadIdx.x; i < (2 * PATCH_BYTES) / 16; i += S_THREADS) sts_v4(sP + i * 16, 0u, 0u, 0u, 0u);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the zero rows / columns of A are read by the tensor core
   __syncthreads();
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(128u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < 4) {
     // ============================== builders ==============================
@@ -193,82 +168,61 @@ psb_stem_fwd_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_con
       if (lane == 0) mbar_arrive(&a_full[buf]);
       named_bar(1, 128);                               // everybody finished READING patch[buf] (refilled during the next tile)
     }
-  } else if (warp == 8) {
-    // ============================== MMA issuer ==============================
-    if (elect_one()) {
-      if (p.ready_flag != nullptr) {       // patch loads / A-tile builds of the first tiles already run in the other warps
+  } else {
+    // ============================== MMA + epilogue ==============================
+    const int et = threadIdx.x - 128;                  // 0..255
+    const int c = et >> 7, wt = et & 127;              // warpgroup c owns pixel rows c*64 .. c*64+63 of the tile
+    const int frow = c * 64 + (wt >> 5) * 16 + ((lane) >> 2), fcol = 2 * (lane & 3);   // fragment origin (wgmma_m64n64)
+    if (et == 0) {
+      if (p.ready_flag != nullptr) {       // patch loads / A-tile builds of the first tiles already run in the builders
         psb::spin_until_ge(p.ready_flag, p.ready_epoch, p.err_slot, p.timeout_ns);
         asm volatile("fence.proxy.async;" ::: "memory");   // generic-proxy acquire → async-proxy (TMA) reads
       }
       mbar_expect_tx(b_full, SB_BYTES);
       for (int b = 0; b < 3; ++b) tma_load_2d(&tmap_w, b_full, smem + OFF_B + b * SB_BLK, b * 64, 0);
     }
-    __syncwarp();
     mbar_wait(b_full, 0);
-    const uint32_t idesc = stem_idesc();
-    for (int t = t0, i = 0; t < t1; ++t, ++i) {
-      const int buf = i & 1;
-      const uint32_t par = (i >> 1) & 1;
-      mbar_wait(&t_empty[buf], par ^ 1);
-      mbar_wait(&a_full[buf], par);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
-        const uint32_t d_tmem = tmem_base + buf * 64;
-#pragma unroll
-        for (int kk = 0; kk < SK / UMMA_K; ++kk) {
-          const uint64_t da = make_desc(sA + buf * SA_BYTES + (kk >> 2) * SA_BLK) + (uint64_t)(2 * (kk & 3));
-          const uint64_t db = make_desc(sB + (kk >> 2) * SB_BLK) + (uint64_t)(2 * (kk & 3));
-          umma(d_tmem, da, db, idesc, kk != 0);
-        }
-        umma_commit(&a_empty[buf]);
-        umma_commit(&t_full[buf]);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ============================== epilogue ==============================
-    const int quarter = warp & 3;                      // warps 4..7 → TMEM lane quarters 0..3
-    const int et = (warp - 4) * 32 + lane;             // 0..127
-    const int row = quarter * 32 + lane;               // == et
-    const int ch = et & 63, half = et >> 6;
-    const int rhalf = (p.OW + 1) >> 1;
-    const int r0 = half * rhalf, r1 = min(p.OW, r0 + rhalf);
+    const int ch = et & 63, part = et >> 6;            // column sums: channel ch over a quarter of the rows
+    const int rq = (p.OW + 3) >> 2;
+    const int r0 = part * rq, r1 = min(p.OW, r0 + rq);
     float s_sum = 0.f, s_sq = 0.f;
+    float acc[32];
     for (int t = t0, i = 0; t < t1; ++t, ++i) {
       const int buf = i & 1;
-      mbar_wait(&t_full[buf], (i >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t r[32], pk[32];
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * 64;
-      tmem_ld_32x32b_x32(taddr, r);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      mbar_wait(&a_full[buf], (i >> 1) & 1);
+      wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < 16; ++j) pk[j] = psb::pack_bf16x2(__uint_as_float(r[2 * j]), __uint_as_float(r[2 * j + 1]));
-      tmem_ld_32x32b_x32(taddr + 32, r);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int j = 0; j < 16; ++j) pk[16 + j] = psb::pack_bf16x2(__uint_as_float(r[2 * j]), __uint_as_float(r[2 * j + 1]));
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&t_empty[buf]);       // the accumulator is free again: the MMAs of tile i+2 may start
+      for (int kk = 0; kk < SK / WG_K; ++kk) {
+        const uint64_t da = make_desc(sA + buf * SA_BYTES + (kk >> 2) * SA_BLK + c * 64 * 128 + 32 * (kk & 3));
+        const uint64_t db = make_desc(sB + (kk >> 2) * SB_BLK + 32 * (kk & 3));
+        wgmma_m64n64<0, 0>(acc, da, db, kk != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (wt == 0) mbar_arrive(&a_empty[buf]);         // A[buf] may be rebuilt for tile i+2
 
       // staging buffer `buf`: the bulk store issued from it two tiles ago must have finished reading it
       if (et == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      named_bar(2, 128);
-      const uint32_t orow = sO + buf * SO_BYTES + row * 128;
+      named_bar(2, 256);
+      const uint32_t so = sO + buf * SO_BYTES;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) sts_v4(orow + ((j ^ (row & 7)) << 4), pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = frow + 8 * h;
+          asm volatile("st.shared.u32 [%0], %1;" ::"r"(so + r * 128 + ((j ^ (r & 7)) << 4) + fcol * 2),
+                       "r"(psb::pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]))
+                       : "memory");
+        }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      named_bar(2, 128);
+      named_bar(2, 256);
       if (et == 0) {
-        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tmap_y),
-                     "r"(sO + buf * SO_BYTES), "r"(0), "r"(t * p.OW)
-                     : "memory");
+        tma_store_2d(&tmap_y, so, 0, t * p.OW);
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       }
       if (p.sums != nullptr) {
         // column sums of the bf16 values just staged (what a separate statistics pass would read back)
-        const uint32_t cbase = sO + buf * SO_BYTES + (ch & 7) * 2;
+        const uint32_t cbase = so + (ch & 7) * 2;
         for (int rr = r0; rr < r1; ++rr) {
           const float v = __uint_as_float(lds_u16(cbase + rr * 128 + (((ch >> 3) ^ (rr & 7)) << 4)) << 16);
           s_sum += v;
@@ -276,32 +230,31 @@ psb_stem_fwd_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_con
         }
       }
     }
-    if (p.sums != nullptr && t0 < t1) {
-      atomicAdd(p.sums + ch, s_sum);
-      atomicAdd(p.sums + 64 + ch, s_sq);
+    if (p.sums != nullptr) {        // the four row quarters of each channel, added in a fixed order: no float atomics
+      __shared__ float red[2][4][64];
+      red[0][part][ch] = s_sum;
+      red[1][part][ch] = s_sq;
+      named_bar(2, 256);
+      if (et < 128) {
+        const float* r = red[et >> 6][0] + ch;
+        p.sums[(size_t)blockIdx.x * 128 + et] = ((r[0] + r[64]) + r[128]) + r[192];
+      }
     }
     if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 8) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128u) : "memory");
   }
 }
 
 // ==========================================================================================================
 // Weight gradient of the stem, implicit too:  dW2d[co][k] = Σ_pixels gy[p][co] · A[p][k].
-// The reduction runs over PIXELS, so both operands are "MN-major" for the tensor core — which is exactly how they
-// already sit in shared memory: the im2col tile built by build_row ([pixel rows][k], k contiguous) is the M-side
-// operand, the TMA-loaded gy tile ([pixel rows][64 channels]) the N-side one.  UMMA M = 128 covers k-blocks {0,1};
-// a second MMA over k-blocks {1,2} provides k = 128..175 (rows 64..111 of its accumulator).  Both accumulators stay
-// in TMEM for the CTA's whole life; each CTA writes one fp32 partial [176][64] and the host sums the partials
-// (deterministic, 148 x 45 KB).
-//   warps 0-3  builders (as in the forward), then the final TMEM → global epilogue
-//   warp  4    TMA producer of the gy tiles     warp 5   MMA issuer
+// The reduction runs over PIXELS, so both operands are MN-major for the tensor core — which is exactly how they already sit
+// in shared memory: the im2col tile built by build_row ([pixel rows][k], k contiguous) is the M-side operand, the TMA-loaded
+// gy tile ([pixel rows][64 channels]) the N-side one.  Three wgmma m64n64k16 per 16 pixels cover k-blocks 0, 1, 2
+// (k = 0..191; k >= 176 is zero).  The accumulators stay in registers for the CTA's whole life; each CTA writes one fp32
+// partial [176][64] and the host sums the partials (deterministic, 132 x 45 KB).
+//   warpgroup 0  builders (as in the forward); thread 0 also TMA-loads the gy tile of the buffer it fills
+//   warpgroup 1  MMA issuer, then the final register → global epilogue
 // ==========================================================================================================
-constexpr int WG_THREADS = 192;
+constexpr int WG_THREADS = 256;
 constexpr int SG_BYTES = 128 * 128;                              // gy tile: up to 128 pixel rows x 64 bf16
 constexpr int WOFF_A = 0;
 constexpr int WOFF_G = WOFF_A + 2 * SA_BYTES;                    // 98 304
@@ -317,20 +270,6 @@ struct StemWgradParams {
   int N, H, W, OH, OW;
 };
 
-// MN-major, SWIZZLE_128B smem descriptor: 64-element MN blocks `lbo` bytes apart, 8-row K groups 1024 bytes apart
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3ffffu) >> 4);
-  d |= (uint64_t)(lbo_bytes >> 4) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t stem_idesc_mn() {   // as stem_idesc, both operands MN-major (bits 15 / 16)
-  return stem_idesc() | (1u << 15) | (1u << 16);
-}
-
 __global__ void __launch_bounds__(WG_THREADS, 1)
 psb_stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ StemWgradParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -338,9 +277,7 @@ psb_stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_c
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WOFF_BAR);
   uint64_t* a_full = bars;            // [2]  4 builder warps arrive
   uint64_t* g_full = bars + 2;        // [2]  TMA bytes of the gy tile
-  uint64_t* empty = bars + 4;         // [2]  tcgen05.commit: A[buf] and G[buf] are free again
-  uint64_t* d_full = bars + 6;        // [1]  every MMA of this CTA has completed
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 7);
+  uint64_t* empty = bars + 4;         // [2]  the wgmmas that read A[buf] and G[buf] have retired
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles = p.N * p.OH;
@@ -356,7 +293,6 @@ psb_stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_c
       mbar_init(&g_full[i], 1);
       mbar_init(&empty[i], 1);
     }
-    mbar_init(d_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   // rows >= OW of A and of the gy tiles take part in the last K step: they must be zero, not stale bits
@@ -364,15 +300,6 @@ psb_stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_c
   for (int i = threadIdx.x; i < (2 * PATCH_BYTES) / 16; i += WG_THREADS) sts_v4(sP + i * 16, 0u, 0u, 0u, 0u);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
-  if (warp == 5) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(128u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
   StemParams lp{};                                     // load_patch only reads x / H / W / OH
   lp.x = p.x, lp.N = p.N, lp.H = p.H, lp.W = p.W, lp.OH = p.OH, lp.OW = p.OW;
 
@@ -390,78 +317,52 @@ psb_stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_c
       }
       named_bar(1, 128);
       mbar_wait(&empty[buf], ((i >> 1) & 1) ^ 1);
+      if (bt == 0) {
+        mbar_expect_tx(&g_full[buf], (uint32_t)p.OW * 128u);
+        tma_load_2d(&tmap_g, &g_full[buf], smem + WOFF_G + buf * SG_BYTES, 0, t * p.OW);
+      }
       if (bt < p.OW) build_row(sP + buf * PATCH_BYTES, sA + buf * SA_BYTES, pitch, bt);
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
       if (lane == 0) mbar_arrive(&a_full[buf]);
       named_bar(1, 128);
     }
-    // ---- final epilogue: this CTA's partial dW2d^T [176][64] ----
-    float* out = p.partial + (size_t)blockIdx.x * SK * 64;
-    const int r = warp * 32 + lane;                    // TMEM lane == accumulator row
-    if (t0 < t1) {
-      mbar_wait(d_full, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-      for (int part = 0; part < 2; ++part) {           // accumulator 0: k = r;  accumulator 1: k = 64 + r (r >= 64 only)
-        const int k = part == 0 ? r : 64 + r;
-#pragma unroll 1
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(warp * 32) << 16) + part * 64 + c0, v);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if ((part == 0 || r >= 64) && k < SK) {
-            float4* o = reinterpret_cast<float4*>(out + (size_t)k * 64 + c0);
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              o[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                 __uint_as_float(v[4 * j + 3]));
-          }
-        }
-      }
-    } else {
-      for (int k = r; k < SK; k += 128)
-        for (int c = 0; c < 64; ++c) out[(size_t)k * 64 + c] = 0.f;
-    }
-  } else if (warp == 4) {
-    // ============================== gy TMA producer ==============================
-    if (elect_one()) {
-      for (int t = t0, i = 0; t < t1; ++t, ++i) {
-        const int buf = i & 1;
-        mbar_wait(&empty[buf], ((i >> 1) & 1) ^ 1);
-        mbar_expect_tx(&g_full[buf], (uint32_t)p.OW * 128u);
-        tma_load_2d(&tmap_g, &g_full[buf], smem + WOFF_G + buf * SG_BYTES, 0, t * p.OW);
-      }
-    }
   } else {
-    // ============================== MMA issuer ==============================
-    const uint32_t idesc = stem_idesc_mn();
-    const int ksteps = (p.OW + 15) >> 4;               // 16 pixel rows per UMMA K step (rows >= OW are zero)
+    // ============================== MMA, then this CTA's partial dW2d^T [176][64] ==============================
+    const int wt = threadIdx.x - 128;
+    const int frow = (wt >> 5) * 16 + (lane >> 2), fcol = 2 * (lane & 3);   // fragment origin (wgmma_m64n64)
+    const int ksteps = (p.OW + 15) >> 4;               // 16 pixel rows per wgmma K step (rows >= OW are zero)
+    float acc[3][32];
     for (int t = t0, i = 0; t < t1; ++t, ++i) {
       const int buf = i & 1;
       const uint32_t par = (i >> 1) & 1;
       mbar_wait(&a_full[buf], par);
       mbar_wait(&g_full[buf], par);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
+      wgmma_fence();
 #pragma unroll 1
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const uint32_t a0 = sA + buf * SA_BYTES + ks * 2048;
-          const uint64_t dg = make_desc_mn(sG + buf * SG_BYTES + ks * 2048, 16);
-          umma(tmem_base, make_desc_mn(a0, SA_BLK), dg, idesc, (i | ks) != 0);                 // k-blocks 0,1 → k 0..127
-          umma(tmem_base + 64, make_desc_mn(a0 + SA_BLK, SA_BLK), dg, idesc, (i | ks) != 0);   // k-blocks 1,2 → k 64..191
-        }
-        umma_commit(&empty[buf]);
-        if (t + 1 == t1) umma_commit(d_full);
+      for (int ks = 0; ks < ksteps; ++ks) {
+        const uint64_t dg = make_desc(sG + buf * SG_BYTES + ks * 2048, SG_BYTES);
+#pragma unroll
+        for (int b = 0; b < 3; ++b)                    // k-block b → k = 64b .. 64b+63
+          wgmma_m64n64<1, 1>(acc[b], make_desc(sA + buf * SA_BYTES + b * SA_BLK + ks * 2048, SA_BLK), dg, (i | ks) != 0);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (wt == 0) mbar_arrive(&empty[buf]);
     }
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 5) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128u) : "memory");
+    float* out = p.partial + (size_t)blockIdx.x * SK * 64;
+#pragma unroll
+    for (int b = 0; b < 3; ++b)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int k = 64 * b + frow + 8 * h;
+        if (k < SK) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<float2*>(out + (size_t)k * 64 + 8 * j + fcol) =
+                t0 < t1 ? make_float2(acc[b][4 * j + 2 * h], acc[b][4 * j + 2 * h + 1]) : make_float2(0.f, 0.f);
+        }
+      }
   }
 }
 
@@ -493,11 +394,22 @@ void psb_stem_wgrad_finalize_launch(cudaStream_t s, const float* partial, int gr
   psb_stem_wgrad_finalize_kernel<<<(SK * 64 + 255) / 256, 256, 0, s>>>(partial, grid, reinterpret_cast<__nv_bfloat16*>(out_bf16));
 }
 
+namespace {
+// sums[j] = Σ_cta part[cta][j] in CTA order (deterministic), j < 128
+__global__ void __launch_bounds__(128) psb_stem_sums_kernel(const float* __restrict__ part, int grid, float* __restrict__ sums) {
+  float acc = 0.f;
+  for (int g = 0; g < grid; ++g) acc += part[(size_t)g * 128 + threadIdx.x];
+  sums[threadIdx.x] = acc;
+}
+
+}  // namespace
+
 int psb_stem_fwd_smem_bytes() { return STEM_SMEM; }
 
 // tmap_w: [64,176] bf16 weights, box 64 x 64, SWIZZLE_128B.  tmap_y: [N*OH*OW, 64] bf16 output, box 64 columns x OW rows,
-// SWIZZLE_128B.  `sums` (nullable) must hold 128 zeroed floats.
-void psb_stem_fwd_launch(cudaStream_t s, const void* tmap_w, const void* tmap_y, const void* x, float* sums, int N, int H, int W,
+// SWIZZLE_128B.  `sums` (nullable): 128 floats, Σy | Σy² per channel; `part`: num_sms x 128 floats of per-CTA partials.
+void psb_stem_fwd_launch(cudaStream_t s, const void* tmap_w, const void* tmap_y, const void* x, float* sums, float* part, int N,
+                         int H, int W,
                          int num_sms, const uint64_t* ready_flag, uint64_t ready_epoch, unsigned long long timeout_ns) {
   static bool configured = false;
   if (!configured) {
@@ -506,7 +418,7 @@ void psb_stem_fwd_launch(cudaStream_t s, const void* tmap_w, const void* tmap_y,
   }
   StemParams p{};
   p.x = reinterpret_cast<const __nv_bfloat16*>(x);
-  p.sums = sums;
+  p.sums = sums != nullptr ? part : nullptr;
   p.N = N, p.H = H, p.W = W;
   p.OH = (H - 1) / 2 + 1, p.OW = (W - 1) / 2 + 1;
   p.ready_flag = ready_flag;
@@ -518,10 +430,14 @@ void psb_stem_fwd_launch(cudaStream_t s, const void* tmap_w, const void* tmap_y,
   psb_count_launch(1);
   psb_stem_fwd_kernel<<<grid, S_THREADS, STEM_SMEM, s>>>(*reinterpret_cast<const CUtensorMap*>(tmap_w),
                                                         *reinterpret_cast<const CUtensorMap*>(tmap_y), p);
+  if (sums != nullptr) {
+    psb_count_launch(1);
+    psb_stem_sums_kernel<<<1, 128, 0, s>>>(part, grid, sums);
+  }
 }
 
 // tmap_g: [N*OH*OW, 64] bf16 output gradient (channels-last), box 64 columns x OW rows, SWIZZLE_128B.
-// `partial`: [grid][176][64] fp32, fully written (no zeroing needed); returns the grid size through *grid_out.
+// `partial`: [grid][176][64] fp32, fully written (no zeroing needed).
 int psb_stem_wgrad_grid(int N, int H, int num_sms) {
   const int tiles = N * ((H - 1) / 2 + 1);
   return tiles < num_sms ? tiles : num_sms;

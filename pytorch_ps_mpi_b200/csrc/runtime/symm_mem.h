@@ -2,7 +2,7 @@
 // driver API: cuMemCreate / export POSIX fd / SCM_RIGHTS fd passing / cuMemImport / cuMemMap,
 // and cuMulticastCreate / AddDevice / BindMem for the switch-replicated alias.
 //
-// This is the B200 stand-in for what libmpi gives the reference (a shared address space for
+// This is the GPU stand-in for what libmpi gives the reference (a shared address space for
 // collectives over host buffers, /root/reference/mpi_comms.py:88,132,162): every rank's gradient
 // wire arena, parameter arena and signal pad are mapped into every process, so one kernel can
 // gather / reduce / broadcast with plain loads and stores over NVLink.  No NCCL, no MPI.

@@ -8,7 +8,7 @@ import torch.nn.functional as F
 
 class MLP(nn.Module):
     """``in → hidden → classes`` with ReLU.  ``first_linear`` can be swapped for the
-    broadcast-fused tcgen05 GEMM (:class:`pytorch_ps_mpi_b200.ops.linear.BcastLinear`)."""
+    broadcast-fused wgmma GEMM (:class:`pytorch_ps_mpi_b200.ops.linear.BcastLinear`)."""
 
     def __init__(self, in_features: int = 784, hidden: int = 512, classes: int = 10, bias: bool = True):
         super().__init__()

@@ -1,4 +1,4 @@
-"""ResNet-18 / ResNet-50 (BASELINE.json configs 2 and 3), written for channels-last bf16 on B200.
+"""ResNet-18 / ResNet-50 (BASELINE.json configs 2 and 3), written for channels-last bf16 on H100.
 
 Plain ``torch.nn`` definition (He et al. 2015 topology, torchvision-compatible parameter
 names so checkpoints interchange).  Convolutions are library (cuDNN) GEMMs — the framework's own
@@ -17,8 +17,8 @@ from ..ops.batchnorm import FusedBatchNormAct2d
 from ..ops.pooling import FusedMaxPool2d
 from ..ops.stem import STEM_K, STEM_STRIDES, stem_conv, stem_conv_fused, stem_fused_supported, stem_supported
 
-# Default since round 2 (validated on B200, bench/stem_fused_check.py): one implicit-GEMM stem kernel with the BatchNorm
-# statistics in its epilogue (csrc/kernels/stem_kernels.cu) instead of im2col + GEMM + statistics pass: 0.97 → 0.47 ms.
+# Default (checked by bench/stem_fused_check.py): one implicit-GEMM stem kernel with the BatchNorm
+# statistics in its epilogue (csrc/kernels/stem_kernels.cu) instead of im2col + GEMM + statistics pass.
 # PSB200_STEM=im2col restores the round-1 path.
 _FUSED_STEM = os.environ.get("PSB200_STEM", "fused").lower() != "im2col"
 
@@ -125,7 +125,7 @@ class ResNet(nn.Module):
         c = self.conv1
         if x.shape[1] == c.in_channels:
             if self.gemm_stem and stem_supported(x, c):
-                return stem_conv(x, c.weight)          # im2col + our tcgen05 GEMM (cuDNN: 2.5 ms/step here)
+                return stem_conv(x, c.weight)          # im2col + our wgmma GEMM (C=3 defeats cuDNN)
             return c(x)
         w = F.pad(c.weight, (0, 0, 0, 0, 0, x.shape[1] - c.in_channels))
         if x.is_contiguous(memory_format=torch.channels_last):

@@ -16,7 +16,7 @@ gather, ``mpi_comms.py:60-117``), ``ibroadcast``/``irecv1`` (PS→worker broadca
 * ``Iallgather.prepare`` exchanges all P sizes in ONE message, not P collectives
   (``mpi_comms.py:150-158``).
 
-This path serves arbitrary Python objects and user codings.  Dense tensors on B200 never come
+This path serves arbitrary Python objects and user codings.  Dense tensors on the GPU never come
 through here: they use the symmetric-memory kernels in :mod:`pytorch_ps_mpi_b200.parallel`.
 """
 from __future__ import annotations

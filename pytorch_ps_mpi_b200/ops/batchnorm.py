@@ -1,8 +1,8 @@
 """``FusedBatchNormAct2d``: BatchNorm2d (+ residual add) (+ ReLU) in hand-written channels-last bf16
 kernels (``csrc/kernels/bn_kernels.cu``), forward and backward.
 
-ATen's channels-last BatchNorm plus the separate add / ReLU kernels are ~45 % of a ResNet-18 step
-on B200 (``profiles/resnet18_step_launches_n1.txt``); fusing them turns 5-6 HBM passes per
+ATen's channels-last BatchNorm plus the separate add / ReLU kernels are a large share of a ResNet-18
+step; fusing them turns 5-6 HBM passes per
 BN-add-ReLU into 3 (forward) and the backward's 4 kernels into 2 passes over ``dy``/``x``.
 
 Same parameters / buffers / ``state_dict`` as ``nn.BatchNorm2d``; running statistics stay fp32 even

@@ -1,4 +1,4 @@
-"""``BcastLinear``: a linear layer whose forward GEMM is the hand-written tcgen05 kernel
+"""``BcastLinear``: a linear layer whose forward GEMM is the hand-written wgmma kernel
 (``csrc/kernels/bcast_gemm.cu``) and whose weight operand is consumed straight out of the
 symmetric parameter arena the parameter server broadcasts into.
 
@@ -52,11 +52,11 @@ class _BcastLinearFn(torch.autograd.Function):
 
 def bcast_linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None, relu: bool = False,
                  w_ptr: int = 0, flag_ptr: int = 0, epoch: int = 0, variant: int = 0) -> torch.Tensor:
-    """``act(x @ weight.T + bias)`` on tcgen05 (bf16 in, fp32 accumulate, bf16 out).
+    """``act(x @ weight.T + bias)`` on wgmma (bf16 in, fp32 accumulate, bf16 out).
 
-    ``variant``: 0 = auto (2-CTA ``cta_group::2`` 256x256 tiles when M >= 256), 1 = 1-CTA, 2 = 2-CTA.  Bits 4-7 select the
-    2-CTA kernel's epilogue (``csrc/kernels/bcast_gemm2.cu``: 0 = auto → TMA store, 1 = staged full-line stores, 3 = TMA store,
-    4 = the round-1 row-strided stores kept for A/B; ``bench/gemm_variants.py``)."""
+    ``variant``: 0 = auto (CTA pairs sharing the weight tile when M >= 256), 1 = one CTA per tile, 2 = CTA pairs.  Bits 4-7
+    select the epilogue (``csrc/kernels/bcast_gemm.cu``: 0 = auto → TMA store, 1 = staged full-line stores, 3 = TMA store,
+    4 = direct stores from the accumulator fragment, kept for A/B; ``bench/gemm_variants.py``)."""
     if not (x.is_cuda and x.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and weight.is_contiguous()
             and weight.shape[1] % 8 == 0):
         y = F.linear(x, weight, bias)          # shapes/dtypes the kernel does not cover
@@ -70,7 +70,7 @@ def bcast_linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Ten
 
 
 class BcastLinear(nn.Linear):
-    """Drop-in ``nn.Linear`` (same parameters / state_dict) running on the tcgen05 GEMM."""
+    """Drop-in ``nn.Linear`` (same parameters / state_dict) running on the wgmma GEMM."""
 
     def __init__(self, in_features, out_features, bias=True, relu=False, **kw):
         super().__init__(in_features, out_features, bias=bias, **kw)
@@ -85,7 +85,7 @@ class BcastLinear(nn.Linear):
         ``gate=True``: the kernel's TMA producer acquires the broadcast epoch itself and workers stop queueing
         the separate wait kernel — only valid when this layer is the FIRST consumer of parameters in the
         forward pass (an MLP's first layer; NOT BERT's first linear, whose embeddings are read earlier).
-        ``gate=False``: the engine keeps its wait kernel; the layer just runs on the tcgen05 GEMM.
+        ``gate=False``: the engine keeps its wait kernel; the layer just runs on the wgmma GEMM.
         ``pull=True``: weight tiles are TMA-loaded from the server's arena over NVLink."""
         eng = getattr(optimizer, "_engine", None)
         if eng is None:

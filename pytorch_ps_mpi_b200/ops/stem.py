@@ -1,9 +1,8 @@
-"""ResNet stem (7x7 / stride 2 / pad 3, 3 → 64 channels) on OUR tcgen05 kernels.
+"""ResNet stem (7x7 / stride 2 / pad 3, 3 → 64 channels) on OUR wgmma kernels.
 
 Default path (round 2): ``stem_conv_fused`` — ONE implicit-GEMM kernel (``psb_stem_fwd_kernel``, ``csrc/kernels/stem_kernels.cu``:
-smem patch → swizzled A tile → ``tcgen05.mma`` → TMA-store epilogue that also produces the BatchNorm Σy / Σy²) and the implicit
-weight gradient ``psb_stem_wgrad_kernel`` (the same A tile as an MN-major operand, accumulators resident in TMEM).  Measured on
-B200 at batch 256: stem + BN 0.97 → 0.47 ms, weight gradient 0.69 → 0.26 ms; no 1.13 GB patch matrix.
+smem patch → swizzled A tile → ``wgmma`` → TMA-store epilogue that also produces the BatchNorm Σy / Σy²) and the implicit
+weight gradient ``psb_stem_wgrad_kernel`` (the same A tile as an MN-major operand, accumulators resident in registers); no 1.13 GB patch matrix.
 
 The convolution weight is kept **in the parameter arena in the [64,176] GEMM layout** the kernel TMA-loads (``STEM_STRIDES``: a
 ``[64,3,7,7]`` view with strides ``(176,1,24,3)``; the device engine honours ``param.ps_arena_layout``), so the parameter
@@ -13,7 +12,7 @@ server's broadcast lands it ready to use and, with ``ResNet.attach(optimizer)``,
 
 Fallback (``PSB200_STEM=im2col``, or widths the fused kernel does not cover): ``stem_conv`` — ``psb_im2col_stem`` builds the
 ``[N*OH*OW, 176]`` patch matrix, the product runs on ``psb_bcast_gemm``, the weight gradient is one library GEMM.
-cuDNN needs 2.5 ms per step for this layer on B200 (C=3 defeats its tensor-core kernels).
+cuDNN is slow on this layer (C=3 defeats its tensor-core kernels).
 """
 from __future__ import annotations
 
@@ -35,7 +34,7 @@ _IMPLICIT_WGRAD = os.environ.get("PSB200_STEM_WGRAD", "implicit").lower() != "im
 class _StemGemm(torch.autograd.Function):
     @staticmethod
     def forward(ctx, a, w2d):
-        y = bcast_linear(a, w2d)                       # [M,176] x [64,176]^T on tcgen05
+        y = bcast_linear(a, w2d)                       # [M,176] x [64,176]^T on wgmma
         ctx.save_for_backward(a)
         return y
 

@@ -1,4 +1,4 @@
-"""Device engine: the B200 hot path behind ``MPI_PS.step()``.
+"""Device engine: the GPU hot path behind ``MPI_PS.step()``.
 
 Per step, per rank (nothing on this path touches the host after the launches are queued, and
 nothing goes through NCCL/MPI):

@@ -52,7 +52,7 @@ class FlatLayout:
             n, strides = p.numel(), None
             # A module may ask for a custom physical placement of its parameter inside the arena
             # (``param.ps_arena_layout = (strides, span_numel)``): e.g. the ResNet stem keeps its [64,3,7,7] weight in the
-            # zero-padded [64,176] GEMM layout its tcgen05 kernel TMA-loads, so the PS broadcast lands the weight directly in
+            # zero-padded [64,176] GEMM layout its wgmma kernel TMA-loads, so the PS broadcast lands the weight directly in
             # the form the first forward GEMM consumes (no per-step re-layout).  Elements of the span the view does not
             # cover are padding: zero, zero gradient, untouched by SGD/Adam (0 stays 0).
             hint = getattr(p, "ps_arena_layout", None)

@@ -731,73 +731,77 @@ def build_async(n: int, epochs: int, quota: int = 1, consistent: bool = False, d
 
 
 def build_stem_pipeline(n: int = 1, epochs: int = 4, drop: Optional[str] = None) -> Model:
-    """Intra-CTA pipeline of the fused stem kernel (``csrc/kernels/stem_kernels.cu::psb_stem_fwd_kernel``):
-    builder warps, the MMA warp, the epilogue warps, the cp.async patch loads and the bulk stores, over ``epochs``
-    tiles.  mbarrier phase waits are modelled as counts (``wait(parity)`` at tile ``i`` of a double-buffered resource
-    == "at least ``i // 2`` completions", exact because nothing can run two phases ahead — which the search confirms by
-    never finding a version mismatch).  ``n`` is unused (one CTA).
+    """Intra-CTA pipeline of the fused stem kernel (``csrc/kernels/stem_kernels.cu::psb_stem_fwd_kernel``): the builder
+    warpgroup (cp.async patch loads + A-tile builds), the two MMA + epilogue warpgroups (wgmma on their 64 rows of A[buf],
+    then staging + BatchNorm column sums from registers) and the TMA unit executing the bulk stores, over ``epochs`` tiles.
+    mbarrier phase waits are modelled as counts (``wait(parity)`` at tile ``i`` of a double-buffered resource == "at least
+    ``i // 2`` completions", exact because nothing can run two phases ahead).  ``a_empty`` takes one arrival per MMA
+    warpgroup (two slots here); named barrier 2 (256 threads) is a pair of sig / wait per warpgroup.  ``n`` is unused.
 
-    ``drop``: ``'a_empty'`` (builders do not wait for the MMAs that read the A buffer), ``'t_empty'`` (the MMA warp does
-    not wait for the epilogue to drain the accumulator), ``'store_wait'`` (the staging tile is rewritten while the bulk
-    store still reads it).  (The named barriers between the four builder warps are below this model's resolution:
-    they are one process here.)"""
+    ``drop``: ``'a_empty'`` (builders do not wait for the wgmmas that read the A buffer), ``'store_wait'`` (the staging
+    tile is rewritten while the bulk store still reads it), ``'staging_bar'`` (no named barrier before the staging writes,
+    so warpgroup 1 does not wait for warpgroup 0's ``cp.async.bulk.wait_group.read``).  (The named barriers between the
+    four builder warps are below this model's resolution: they are one process here.)"""
     m = Model()
     T = epochs
-    builder, mma, epi, store = [], [], [], []
+    builder, store = [], []
+    cons = [[], []]
     for i in range(T):
         b = i & 1
         k = i // 2
-        # ---- builders (4 warps in lock step through named barriers) ----
+        # ---- builders (4 warps in lock step through named barrier 1) ----
         if i == 0:
             builder.append(("acq", [(("patch", 0), "w", None)]))                    # load_patch(t0)
         if i + 1 < T:
             builder.append(("acq", [(("patch", b ^ 1), "w", None)]))                  # cp.async of tile i+1
         builder.append(("rel", [(("patch", b), "w", i)]))                            # cp.async.wait_group + barrier
         if drop != "a_empty":
-            builder.append(("wait", ("a_empty", b), k))
+            builder.append(("wait", ("a_empty", b, 0), k))
+            builder.append(("wait", ("a_empty", b, 1), k))
         builder.append(("acq", [(("patch", b), "r", i), (("A", b), "w", None)]))     # build_row
         builder.append(("rel", [(("patch", b), "r", None), (("A", b), "w", i)]))
         builder.append(("sig", ("a_full", b), k + 1))
-        # ---- MMA warp ----
-        if drop != "t_empty":
-            mma.append(("wait", ("t_empty", b), k))
-        mma.append(("wait", ("a_full", b), k + 1))
-        mma.append(("acq", [(("A", b), "r", i), (("T", b), "w", None)]))
-        mma.append(("rel", [(("A", b), "r", None), (("T", b), "w", i)]))             # tcgen05.commit fires when they finish
-        mma.append(("sig", ("a_empty", b), k + 1))
-        mma.append(("sig", ("t_full", b), k + 1))
-        # ---- epilogue warps ----
-        epi.append(("wait", ("t_full", b), k + 1))
-        epi.append(("acq", [(("T", b), "r", i)]))
-        epi.append(("rel", [(("T", b), "r", None)]))
-        epi.append(("sig", ("t_empty", b), k + 1))
-        if drop != "store_wait" and i >= 2:
-            epi.append(("wait", ("st_done",), i - 1))                                 # cp.async.bulk.wait_group.read 1
-        epi.append(("acq", [(("O", b), "w", None)]))
-        epi.append(("rel", [(("O", b), "w", i)]))
-        epi.append(("sig", ("st_issued",), i + 1))
-        epi.append(("acq", [(("O", b), "r", i)]))                                     # BatchNorm column sums
-        epi.append(("rel", [(("O", b), "r", None)]))
+        # ---- MMA + epilogue warpgroups c = 0, 1 ----
+        for c in range(2):
+            q = cons[c]
+            q.append(("wait", ("a_full", b), k + 1))
+            q.append(("acq", [(("A", b), "r", i)]))                                  # wgmma + wait_group 0
+            q.append(("rel", [(("A", b), "r", None)]))
+            q.append(("sig", ("a_empty", b, c), k + 1))
+            if c == 0 and drop != "store_wait" and i >= 2:
+                q.append(("wait", ("st_done",), i - 1))                              # cp.async.bulk.wait_group.read 1
+            if drop != "staging_bar":
+                q.append(("sig", ("bar_pre", c), i + 1))                              # named barrier 2
+                q.append(("wait", ("bar_pre", 1 - c), i + 1))
+            q.append(("acq", [(("O", b, c), "w", None)]))                              # this warpgroup's 64 staged rows
+            q.append(("rel", [(("O", b, c), "w", i)]))
+            q.append(("sig", ("bar_post", c), i + 1))                                 # named barrier 2
+            q.append(("wait", ("bar_post", 1 - c), i + 1))
+            if c == 0:
+                q.append(("sig", ("st_issued",), i + 1))
+            q.append(("acq", [(("O", b, 0), "r", i), (("O", b, 1), "r", i)]))       # BatchNorm column sums (all rows)
+            q.append(("rel", [(("O", b, 0), "r", None), (("O", b, 1), "r", None)]))
         # ---- the TMA unit executing the bulk stores, in order ----
         store.append(("wait", ("st_issued",), i + 1))
-        store.append(("acq", [(("O", b), "r", i)]))
-        store.append(("rel", [(("O", b), "r", None)]))
+        store.append(("acq", [(("O", b, 0), "r", i), (("O", b, 1), "r", i)]))
+        store.append(("rel", [(("O", b, 0), "r", None), (("O", b, 1), "r", None)]))
         store.append(("sig", ("st_done",), i + 1))
     m.add("builders", builder)
-    m.add("mma", mma)
-    m.add("epilogue", epi)
+    m.add("mma_epi_0", cons[0])
+    m.add("mma_epi_1", cons[1])
     m.add("tma_store", store)
     return m
 
 
 def build_stem_wgrad_pipeline(n: int = 1, epochs: int = 4, drop: Optional[str] = None) -> Model:
-    """Intra-CTA pipeline of ``psb_stem_wgrad_kernel``: builders + the gy TMA producer fill (A, G)[buf]; the MMA warp
-    accumulates every tile into one TMEM-resident accumulator and frees the pair with one commit; the builders read the
-    accumulator after the last commit.  ``drop``: ``'empty'`` (producers do not wait for the MMAs), ``'d_full'``
-    (the final epilogue does not wait for the last MMA)."""
+    """Intra-CTA pipeline of ``psb_stem_wgrad_kernel``: the builder warpgroup fills A[buf] and its thread 0 issues the gy
+    TMA load into G[buf] after the ``empty`` wait (the TMA unit is a process of its own); the MMA warpgroup accumulates every
+    tile into register-resident accumulators, frees the pair after ``wgmma.wait_group 0`` and finally writes the CTA's
+    partial from its registers (program order, no barrier).  ``drop``: ``'empty'`` (the builders do not wait for the wgmmas
+    before refilling A and G), ``'g_full'`` (the MMA warpgroup does not wait for the gy bytes)."""
     m = Model()
     T = epochs
-    builder, prod, mma = [], [], []
+    builder, gtma, mma = [], [], []
     for i in range(T):
         b, k = i & 1, i // 2
         if i == 0:
@@ -807,25 +811,22 @@ def build_stem_wgrad_pipeline(n: int = 1, epochs: int = 4, drop: Optional[str] =
         builder.append(("rel", [(("patch", b), "w", i)]))
         if drop != "empty":
             builder.append(("wait", ("empty", b), k))
-            prod.append(("wait", ("empty", b), k))
+        builder.append(("sig", ("g_issue", b), k + 1))                               # thread 0: expect_tx + TMA load
         builder.append(("acq", [(("patch", b), "r", i), (("A", b), "w", None)]))
         builder.append(("rel", [(("patch", b), "r", None), (("A", b), "w", i)]))
         builder.append(("sig", ("a_full", b), k + 1))
-        prod.append(("acq", [(("G", b), "w", None)]))                                 # cp.async.bulk.tensor load of gy
-        prod.append(("rel", [(("G", b), "w", i)]))
-        prod.append(("sig", ("g_full", b), k + 1))
+        gtma.append(("wait", ("g_issue", b), k + 1))
+        gtma.append(("acq", [(("G", b), "w", None)]))                                 # cp.async.bulk.tensor load of gy
+        gtma.append(("rel", [(("G", b), "w", i)]))
+        gtma.append(("sig", ("g_full", b), k + 1))
         mma.append(("wait", ("a_full", b), k + 1))
-        mma.append(("wait", ("g_full", b), k + 1))
-        mma.append(("acq", [(("A", b), "r", i), (("G", b), "r", i), (("D",), "w", None)]))
-        mma.append(("rel", [(("A", b), "r", None), (("G", b), "r", None), (("D",), "w", i + 1)]))
+        if drop != "g_full":
+            mma.append(("wait", ("g_full", b), k + 1))
+        mma.append(("acq", [(("A", b), "r", i), (("G", b), "r", i)]))
+        mma.append(("rel", [(("A", b), "r", None), (("G", b), "r", None)]))
         mma.append(("sig", ("empty", b), k + 1))
-    mma.append(("sig", ("d_full",), 1))
-    if drop != "d_full":
-        builder.append(("wait", ("d_full",), 1))
-    builder.append(("acq", [(("D",), "r", T)]))                                       # the CTA's partial dW
-    builder.append(("rel", [(("D",), "r", None)]))
     m.add("builders", builder)
-    m.add("gy_tma", prod)
+    m.add("gy_tma", gtma)
     m.add("mma", mma)
     return m
 

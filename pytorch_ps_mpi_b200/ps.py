@@ -20,7 +20,7 @@ What is new (see DESIGN.md): three *modes* — ``'ps'`` (rank-0 parameter server
 step → broadcast, the README plan ``README.md:37-46``), ``'allgather'`` (the replicated scheme
 the reference actually wires, ``ps.py:140-190``) and ``'async'`` (AsySG-InCon,
 ``README.md:56-81``) — and two *engines*: the device engine
-(:mod:`pytorch_ps_mpi_b200.parallel.device_engine`: symmetric-memory arenas + fused sm_100a
+(:mod:`pytorch_ps_mpi_b200.parallel.device_engine`: symmetric-memory arenas + fused sm_90a
 kernels, used automatically for CUDA parameters with a built-in coding) and the host engine
 below (generic Python objects / user codings over the shm / gloo transport; also the CPU
 plumbing configuration).

@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Regenerate the committed SASS evidence from the built objects (CPU only, needs cuobjdump):
+"""Write SASS evidence of the built objects into ``profiles/sm90a/`` (git-ignored; CPU only, needs cuobjdump):
 
     python scripts/dump_sass.py            # after __graft_entry__.build()
 
-* ``profiles/sass/<kernel>.sass``         the full listing of one instantiation of every named hot-path kernel
-* ``profiles/sass_mnemonics_<obj>.txt``   opcode histogram per object file (what proves tcgen05 / TMA / multimem: UTCHMMA(.2CTA),
-                                          UTMALDG / UTMASTG, LDTM, UTCBAR…MULTICAST, LDGMC…HPADD (multimem.ld_reduce), *.STRONG.SYS)
+* ``profiles/sm90a/sass/<kernel>.sass``   the full listing of one instantiation of every named hot-path kernel
+* ``profiles/sm90a/sass_mnemonics_<obj>.txt`` opcode histogram per object file (what proves wgmma / TMA / multimem: HGMMA,
+                                          UTMALDG(.MULTICAST) / UTMASTG, LDGMC…HPADD (multimem.ld_reduce), *.STRONG.SYS)
 """
 import collections
 import os
@@ -15,7 +15,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OBJ = os.path.join(ROOT, "pytorch_ps_mpi_b200", "_build")
-OUT = os.path.join(ROOT, "profiles")
+OUT = os.path.join(ROOT, "profiles", "sm90a")
 
 # (object, regex on the demangled function header, output name)
 KERNELS = [
@@ -24,8 +24,8 @@ KERNELS = [
     ("ps_kernels.o", r"psb_encode_kernel<2, 1>", "psb_encode_kernel_topk_bf16"),
     ("ps_kernels.o", r"psb_select_kernel", "psb_select_kernel"),
     ("ps_kernels.o", r"psb_snapshot_fetch", "psb_snapshot_fetch"),
-    ("bcast_gemm2.o", r"psb_bcast_gemm2_kernel<256, 3, 0>", "psb_bcast_gemm2_kernel_256_tma_store"),
-    ("bcast_gemm.o", r"psb_bcast_gemm_kernel", "psb_bcast_gemm_kernel_1cta"),
+    ("bcast_gemm.o", r"psb_bcast_gemm_kernel<128, 2, 3>", "psb_bcast_gemm_kernel_pair_tma_store"),
+    ("bcast_gemm.o", r"psb_bcast_gemm_kernel<128, 1, 3>", "psb_bcast_gemm_kernel_1cta_tma_store"),
     ("stem_kernels.o", r"psb_stem_fwd_kernel", "psb_stem_fwd_kernel"),
     ("stem_kernels.o", r"psb_stem_wgrad_kernel", "psb_stem_wgrad_kernel"),
     ("bn_kernels.o", r"psb_bn_bwd_reduce<true, true>", "psb_bn_bwd_reduce_relu_masked"),

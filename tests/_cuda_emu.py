@@ -275,10 +275,10 @@ def rewrite_launches(text: str):
 
 CUDA_RT_SHIM = r'''
 static inline int emu_cudaGetDevice(int* d) { *d = 0; return 0; }
-// the "GPU" has emu_sm_count SMs (148 = B200).  Tests shrink it so that the launchers' grid caps bind on small tensors and the
+// the "GPU" has emu_sm_count SMs (132 = H100).  Tests shrink it so that the launchers' grid caps bind on small tensors and the
 // kernels' grid-stride loops run more than one iteration per CTA — on hardware that is the normal case (ResNet-18: 14 336 pool rows
-// on 2 368 CTAs).  Weak: one copy shared by every emulated translation unit of a library.
-__attribute__((weak)) int emu_sm_count = 148;
+// on 2 112 CTAs).  Weak: one copy shared by every emulated translation unit of a library.
+__attribute__((weak)) int emu_sm_count = 132;
 extern "C" __attribute__((weak)) void emu_set_sm_count(int n) { emu_sm_count = n; }
 static inline int emu_cudaDeviceGetAttribute(int* v, int, int) { *v = emu_sm_count; return 0; }
 static inline int emu_cudaMemsetAsync(void* p, int v, size_t n, cudaStream_t) { memset(p, v, n); return 0; }
@@ -425,7 +425,7 @@ def bn_source(define_count_launch: bool = True) -> str:
 
 def pool_source(define_count_launch: bool = True) -> str:
     """``pool_kernels.cu`` (max-pool, input normalisers, stem im2col: kernels + launchers) plus the one plain-CUDA kernel of
-    ``stem_kernels.cu`` (Σ of the weight-gradient partials; everything else there is tcgen05 / TMA)."""
+    ``stem_kernels.cu`` (Σ of the weight-gradient partials; everything else there is wgmma / TMA)."""
     src = open(os.path.join(KDIR, "pool_kernels.cu")).read()
     body = src[src.index('#include "kernels.h"') + len('#include "kernels.h"'):]
     for fn in ("cudaGetDevice", "cudaDeviceGetAttribute"):
@@ -499,7 +499,7 @@ def bindings_source() -> str:
     for inc in ("#include <ATen/cuda/CUDAContext.h>\n", "#include <c10/cuda/CUDAGuard.h>\n", "#include <c10/cuda/CUDAStream.h>\n",
                 '#include "symm_mem.h"\n'):
         src = drop(src, inc)
-    # no CUDA runtime underneath: launches cannot fail, there is one "stream", 148 "SMs"
+    # no CUDA runtime underneath: launches cannot fail, there is one "stream", emu_sm_count "SMs"
     src = src.replace('#include "kernels.h"\n', '#include "kernels.h"\n#define cudaGetLastError() cudaSuccess\n'
                       '#define cudaGetDevice(p) (*(p) = 0)\nextern int emu_sm_count;\n#define cudaDeviceGetAttribute(p, a, d) (*(p) = emu_sm_count)\n', 1)
     src = drop(src, "c10::cuda::getCurrentCUDAStream().stream()").replace("cudaStream_t cur_stream() { return ; }",
@@ -513,7 +513,7 @@ def bindings_source() -> str:
 
 
 GEMM_STANDINS = r"""
-// ---- the tensor-core kernels (tcgen05 / TMEM / TMA) are NOT emulated: reference math through ATen with the same contract ----
+// ---- the tensor-core kernels (wgmma / TMA) are NOT emulated: reference math through ATen with the same contract ----
 at::Tensor bcast_gemm(const at::Tensor& x, uint64_t w_ptr, int64_t N, int64_t K, c10::optional<at::Tensor> bias, bool relu,
                       uint64_t flag_ptr, uint64_t epoch, double timeout_s, int variant) {
   TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.size(1) == K, "x must be [M,K] bf16");

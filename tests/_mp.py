@@ -440,7 +440,7 @@ def symm_arena(rank, size):
 
 
 def gpu_bcast_linear(rank, size, pull):
-    """MLP whose first GEMM is the tcgen05 kernel gated on the PS broadcast (and optionally PULLING the
+    """MLP whose first GEMM is the wgmma kernel gated on the PS broadcast (and optionally PULLING the
     weight tiles from the server's arena over NVLink)."""
     ps, w = _world(rank, size)
     from pytorch_ps_mpi_b200.models import mnist_mlp

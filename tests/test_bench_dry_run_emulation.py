@@ -3,7 +3,7 @@
 Everything below ``bench.build()`` is the real code: world set-up, NUMA binding attempt, warm-up until stable (collective
 decision), the device-timed arm with per-step events, the end-to-end arm with its static double-buffered inputs, the re-measure
 rule, the cross-rank parameter digest, the clock summary and the JSON line.  The model is the package's ResNet cut down to one
-stage on 32 x 32 images (``bench.build`` is replaced: the emulator is ~10^5 times slower than a B200), the engine and the fused ops
+stage on 32 x 32 images (``bench.build`` is replaced: the emulator is ~10^5 times slower than an H100), the engine and the fused ops
 run over ``_psb200_emu`` (real bindings on emulated kernels, see ``test_model_integration_emulation.py``), ``torch.cuda`` events are
 wall-clock fakes, ranks are threads."""
 import contextlib
@@ -209,3 +209,40 @@ def test_bench_reference_arm_reports_unavailable(monkeypatch, capsys):
     assert bench.main() == 0
     out = json.loads(capsys.readouterr().out.strip().splitlines()[-1])
     assert out["impl"] == "reference" and "unavailable" in out
+
+
+def test_bench_dump_outputs_are_the_same_every_run(bench_env, monkeypatch, capsys, tmp_path):
+    """``--dump-outputs``: the last timed step's loss and every parameter, float32, and two runs with the same arguments write
+    the same bytes."""
+    import numpy as np
+    bench, extm = bench_env
+    runs = []
+    for r in range(2):
+        d = tmp_path / f"run{r}"
+        _run_bench(bench, extm, 1, ["--steps", "2", "--warmup", "3", "--batch", "2", "--no-comparators", "--dump-outputs", str(d)],
+                   monkeypatch, capsys)
+        assert sorted(p.name for p in d.iterdir()) == ["loss.npy", "params.npy"]
+        arrs = {n: np.load(d / n) for n in ("loss.npy", "params.npy")}
+        assert all(a.dtype == np.float32 for a in arrs.values())
+        assert arrs["loss.npy"].shape == (1,) and np.isfinite(arrs["loss.npy"]).all()
+        assert arrs["params.npy"].size == sum(p.numel() for p in MI._tiny_resnet().parameters())
+        runs.append(arrs)
+    for n in runs[0]:
+        assert np.array_equal(runs[0][n], runs[1][n]), n
+
+
+def test_dump_outputs_of_a_large_model_stay_within_64_mb(tmp_path):
+    """Above ``DUMP_MAX_ELEMS`` parameters the dump is a fixed seeded sample with its indices, 48 MB + the loss at most."""
+    import numpy as np
+    import bench
+    torch.manual_seed(0)
+    model = torch.nn.Linear(4096, 3300)                                   # 13.5 M parameters > DUMP_MAX_ELEMS
+    flat = torch.cat([p.detach().flatten() for p in model.parameters()])
+    for d in (tmp_path / "a", tmp_path / "b"):
+        bench.dump_outputs(str(d), model, torch.tensor(1.5))
+    total = sum(p.stat().st_size for p in (tmp_path / "a").iterdir())
+    assert total <= 64 << 20, total
+    vals, idx = np.load(tmp_path / "a" / "params.npy"), np.load(tmp_path / "a" / "params_index.npy")
+    assert vals.dtype == np.float32 and idx.dtype == np.float64 and vals.shape == idx.shape and 0 < vals.size <= bench.DUMP_SAMPLE
+    assert np.array_equal(vals, flat.numpy()[idx.astype(np.int64)])
+    assert np.array_equal(idx, np.load(tmp_path / "b" / "params_index.npy"))

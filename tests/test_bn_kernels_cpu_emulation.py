@@ -20,9 +20,11 @@ def _single_threaded_torch():
     torch.set_num_threads(n)
 
 DRIVER = r'''
+#include <vector>
 extern "C" void emu_bn_forward(const void* x, const void* res, const void* gamma, const void* beta, void* y, float* scratch /*6C*/,
                                float* rm, float* rv, long long pixels, int C, float eps, float mom, int relu, void* mask) {
-  psb_bn_forward(0, x, res, gamma, beta, y, scratch, scratch + 2 * C, scratch + 3 * C, scratch + 4 * C, scratch + 5 * C, rm, rv, pixels, C,
+  std::vector<float> part(psb_bn_partial_floats(pixels, C));
+  psb_bn_forward(0, x, res, gamma, beta, y, part.data(), scratch + 2 * C, scratch + 3 * C, scratch + 4 * C, scratch + 5 * C, rm, rv, pixels, C,
                  eps, mom, relu, 1, mask);
 }
 extern "C" void emu_bn_forward_presummed(const void* x, const void* gamma, const void* beta, void* y, const float* sums,
@@ -34,7 +36,8 @@ extern "C" void emu_bn_forward_presummed(const void* x, const void* gamma, const
 extern "C" void emu_bn_backward(const void* dy, const void* x, const void* y, const void* gamma, const float* mean, const float* rstd,
                                 float* scratch /*5C*/, void* dx, void* dres, void* dgamma, void* dbeta, long long pixels, int C, int relu,
                                 const void* mask) {
-  psb_bn_backward(0, dy, x, y, gamma, mean, rstd, scratch, scratch + 2 * C, dx, dres, dgamma, dbeta, pixels, C, relu, mask);
+  std::vector<float> part(psb_bn_partial_floats(pixels, C));
+  psb_bn_backward(0, dy, x, y, gamma, mean, rstd, part.data(), scratch + 2 * C, dx, dres, dgamma, dbeta, pixels, C, relu, mask);
 }
 '''
 

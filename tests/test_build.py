@@ -1,5 +1,5 @@
-"""The native extensions exist, import on a CPU-only box, and the CUDA objects really are sm_100a code
-using the Blackwell paths (SASS mnemonics, B200_PROFILING.md §"What proves a Blackwell-native kernel")."""
+"""The native extensions exist, import on a CPU-only box, and the CUDA objects really are sm_90a code
+using the Hopper paths (wgmma, TMA loads / multicast / stores in the SASS)."""
 import shutil
 import subprocess
 
@@ -30,32 +30,31 @@ def _sass(obj):
     return subprocess.run([exe, "-sass", str(obj)], stdout=subprocess.PIPE, text=True, check=True).stdout
 
 
-def test_sass_shows_blackwell_paths():
-    gemm, gemm2, psk = ext.OBJ / "bcast_gemm.o", ext.OBJ / "bcast_gemm2.o", ext.OBJ / "ps_kernels.o"
-    if not gemm.exists() or not psk.exists() or not gemm2.exists():
+def test_sass_shows_hopper_paths():
+    gemm, psk = ext.OBJ / "bcast_gemm.o", ext.OBJ / "ps_kernels.o"
+    if not gemm.exists() or not psk.exists():
         pytest.skip("object files not present (built elsewhere)")
-    s = _sass(gemm) + _sass(gemm2)
-    assert "sm_100a" in s or "SM100" in s.upper() or "EF_CUDA_SM100" in s
-    for mnemonic in ("UTCHMMA", "UTCHMMA.2CTA", "UTMALDG.2D", "UTMALDG.2D.2CTA", "LDTM", "UTCBAR.2CTA.MULTICAST"):
+    s = _sass(gemm)
+    assert "sm_90a" in s or "EF_CUDA_SM90" in s
+    for mnemonic in ("HGMMA.64x128x16.F32.BF16", "HGMMA.64x64x16.F32.BF16", "UTMALDG.2D", "UTMALDG.2D.MULTICAST", "UTMASTG.2D"):
         assert mnemonic in s, f"{mnemonic} missing from bcast_gemm SASS"
     p = _sass(psk)
     assert "STRONG.SYS" in p            # system-scope peer loads/stores of the gather / broadcast
-    ptx_like = subprocess.run(["strings", str(psk)], stdout=subprocess.PIPE, text=True).stdout
-    assert "HMMA" not in s.replace("UTCHMMA", "")      # no legacy mma.sync tensor path in the GEMM
+    assert "HMMA" not in s.replace("HGMMA", "")        # no legacy mma.sync tensor path in the GEMM
 
 
 def test_sass_of_the_fused_stem_and_gemm_epilogues():
-    """The fused stem and the cta_group::2 GEMM (TMA-store epilogue) are real tcgen05 / TMA code, and spill nothing."""
-    stem, gexp = ext.OBJ / "stem_kernels.o", ext.OBJ / "bcast_gemm2.o"
-    if not stem.exists() or not gexp.exists():
+    """The fused stem and the GEMM (TMA-store epilogue) are real wgmma / TMA code, and spill nothing."""
+    stem, gemm = ext.OBJ / "stem_kernels.o", ext.OBJ / "bcast_gemm.o"
+    if not stem.exists() or not gemm.exists():
         pytest.skip("object files not present (built elsewhere)")
     s = _sass(stem)
-    for mnemonic in ("UTCHMMA", "UTMALDG.2D", "UTMASTG.2D", "LDTM", "LDGSTS"):
+    for mnemonic in ("HGMMA.64x64x16.F32.BF16", "UTMALDG.2D", "UTMASTG.2D", "LDGSTS"):
         assert mnemonic in s, f"{mnemonic} missing from stem_kernels SASS"
-    g = _sass(gexp)
-    for mnemonic in ("UTCHMMA.2CTA", "UTMALDG.2D.2CTA", "UTMASTG.2D", "LDTM"):
-        assert mnemonic in g, f"{mnemonic} missing from bcast_gemm_exp SASS"
-    for log in ("stem_kernels.nvcc.log", "bcast_gemm2.nvcc.log", "bcast_gemm.nvcc.log", "bn_kernels.nvcc.log", "pool_kernels.nvcc.log"):
+    g = _sass(gemm)
+    for mnemonic in ("HGMMA.64x128x16.F32.BF16", "UTMALDG.2D.MULTICAST", "UTMASTG.2D"):
+        assert mnemonic in g, f"{mnemonic} missing from bcast_gemm SASS"
+    for log in ("stem_kernels.nvcc.log", "bcast_gemm.nvcc.log", "bn_kernels.nvcc.log", "pool_kernels.nvcc.log"):
         p = ext.OBJ / log
         if p.exists():
             for line in p.read_text().splitlines():
@@ -64,20 +63,21 @@ def test_sass_of_the_fused_stem_and_gemm_epilogues():
 
 
 def test_ps_kernels_spill_budget():
-    """``ps_kernels.cu`` at ``__launch_bounds__(256, 3)`` (85 registers): nothing spills except the fp32-wire Adam instantiation
-    of the update kernel (four fp32 state vectors + two 16-byte gathers per rank in flight), and that one stays under 128 bytes."""
+    """``ps_kernels.cu`` at ``__launch_bounds__(256, 3)`` (85 registers, so that the whole grid is co-resident): nothing spills
+    except the dense-coding update kernels with a 32- or 16-bit wire (fp32 / bf16 / fp16 gathers per rank in flight), and those
+    no more than sm_90a's ptxas spills today: 80 bytes with an fp32 wire, 16 bytes with a bf16 / fp16 wire."""
     p = ext.OBJ / "ps_kernels.nvcc.log"
     if not p.exists():
         pytest.skip("build log not present (built elsewhere)")
-    entry, seen = None, 0
+    budget = {"psb_update_kernelILi0ELi0E": 80, "psb_update_kernelILi0ELi1E": 16, "psb_update_kernelILi0ELi2E": 16}
+    entry = None
     for line in p.read_text().splitlines():
         if "Compiling entry function" in line:
             entry = line.split("'")[1]
         if "spill" in line and "0 bytes spill stores, 0 bytes spill loads" not in line:
-            seen += 1
-            assert "psb_update_kernelILi0ELi0ELi1E" in entry, f"{entry}: {line.strip()}"
-            assert int(line.split("bytes stack frame,")[1].split("bytes spill stores")[0]) <= 128, line
-    assert seen <= 1
+            limit = next((v for k, v in budget.items() if k in entry), None)
+            assert limit is not None, f"{entry}: {line.strip()}"
+            assert int(line.split("bytes stack frame,")[1].split("bytes spill stores")[0]) <= limit, f"{entry}: {line.strip()}"
 
 
 def test_built_extensions_are_not_older_than_their_sources():

@@ -1,8 +1,7 @@
 """GPU tests of the fused ResNet stem (implicit-GEMM forward with BN statistics in the epilogue, implicit weight
-gradient), and every epilogue of the cta_group::2 GEMM.
+gradient), and every epilogue of the GEMM.
 
-First run on a B200 in round 2 (``scratch/round2_first_call.sh`` → 29 passed) and part of the default ``pytest -m gpu``
-run since.  Each compares the kernel with a plain PyTorch fp32 reference of the same op.
+Part of the default ``pytest -m gpu`` run.  Each compares the kernel with a plain PyTorch fp32 reference of the same op.
 """
 import copy
 

@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM / TMA GEMM (``bcast_gemm``) vs a plain PyTorch fp32 reference of the same op."""
+"""wgmma / TMA GEMM (``bcast_gemm``) vs a plain PyTorch fp32 reference of the same op."""
 import pytest
 import torch
 

@@ -2,7 +2,7 @@
 ``ops.batchnorm`` / ``ops.pooling`` / ``ops.stem`` autograd functions with direct gradient placement, driven by 2 ranks of the real
 device engine — over ``_psb200_emu``, the repository's own ``bindings.cpp`` + ``gemm_bindings.cpp`` linked against the emulated
 kernels (``tests/_cuda_emu.py``: BatchNorm, max-pool, im2col, wgrad finalize and every PS kernel are the real source; the three
-tcgen05 entry points are ATen reference math with the same contract).
+tensor-core entry points are ATen reference math with the same contract).
 
 ``Tensor.is_cuda`` is patched to ``True`` for the duration of a test so that the package takes its device paths with host
 tensors; nothing in the package is changed for this."""

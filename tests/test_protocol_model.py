@@ -74,13 +74,13 @@ def test_cli(capsys):
 
 @pytest.mark.parametrize("mode,tiles", [("stem_pipeline", 6), ("stem_wgrad_pipeline", 6)])
 def test_kernel_pipelines_hold(mode, tiles):
-    """The mbarrier hand-offs inside the experimental fused-stem kernels (double-buffered A / patch / staging / TMEM)."""
+    """The mbarrier / named-barrier hand-offs inside the fused-stem kernels (double-buffered patch / A / gy / staging)."""
     res = pm.check(mode, 1, tiles)
     assert res.finals == 1
 
 
-@pytest.mark.parametrize("mode,drop", [("stem_pipeline", "a_empty"), ("stem_pipeline", "t_empty"), ("stem_pipeline", "store_wait"),
-                                       ("stem_wgrad_pipeline", "empty"), ("stem_wgrad_pipeline", "d_full")])
+@pytest.mark.parametrize("mode,drop", [("stem_pipeline", "a_empty"), ("stem_pipeline", "store_wait"), ("stem_pipeline", "staging_bar"),
+                                       ("stem_wgrad_pipeline", "empty"), ("stem_wgrad_pipeline", "g_full")])
 def test_kernel_pipeline_mutants_are_caught(mode, drop):
     with pytest.raises(pm.Violation) as ei:
         pm.check(mode, 1, 5, drop=drop)

@@ -2,7 +2,7 @@
 
 The kernels cannot run here, but their index arithmetic can be checked: this test re-states, byte for byte, what
 ``load_patch`` + ``build_row`` write (zero-margined input rows → 16-byte chunks at swizzled positions of three
-128-row x 128-byte k-blocks) and decodes the result with the CANONICAL UMMA layouts documented in CUTLASS
+128-row x 128-byte k-blocks) and decodes the result with the CANONICAL wgmma layouts documented in CUTLASS
 (``cute/atom/mma_traits_sm100.hpp``):
 
 * K-major  SWIZZLE_128B: ``Swizzle<3,4,3> o ((8,m),(T,2)):((8T,SBO),(1,T))``          — the forward's A operand,
