@@ -158,19 +158,28 @@ class Identity(Coding):
 
 
 def _sat_cast(x: torch.Tensor, wire: int) -> torch.Tensor:
-    """Round-to-nearest-even cast with saturation to the finite range (``cvt.rn.satfinite``)."""
+    """Cast to the wire type by the rules of ``DESIGN.md`` (wire numerics): round to nearest even; narrowing to fp16 / fp8 /
+    int8 saturates finite values and +-Inf at +-max finite; a wire of the tensor's own dtype is an exact copy; NaN stays NaN
+    (int8: the code -128)."""
     dt = _WIRE_TORCH[wire]
+    if x.dtype == dt:
+        return x
     if wire in (WIRE_E4M3, WIRE_E5M2, WIRE_F16):
         m = _WIRE_MAX[wire]
-        x = x.float().clamp(-m, m)
-        return x.to(dt)
+        return x.float().clamp(-m, m).to(dt)         # clamp keeps NaN
     if wire == WIRE_I8:
-        return x.float().round().clamp(-127, 127).to(torch.int8)
+        r = x.float().round().clamp(-127, 127)       # torch.round: ties to even
+        return torch.where(torch.isnan(r), torch.full_like(r, -128.0), r).to(torch.int8)   # no NaN -> int conversion
     return x.to(dt)
 
 
 class Cast(Coding):
-    """Down-cast the gradient to a narrower float on the wire (bf16 / fp16 / fp8)."""
+    """Down-cast the gradient to a narrower float on the wire (bf16 / fp16 / fp8).
+
+    Round to nearest even.  fp16 and fp8 wires saturate finite values and +-Inf at +-max finite (e4m3 448, e5m2 57344,
+    fp16 65504) when they narrow the gradient; bf16 and fp32 wires do not saturate (an fp32 value past the bf16 range
+    becomes Inf).  A wire of the gradient's own dtype is an exact copy, Inf and NaN included.  NaN stays NaN.
+    """
 
     cheap = True
 
@@ -196,8 +205,10 @@ class Cast(Coding):
 class Scale(Coding):
     """Per-tensor abs-max scaling into a narrow type (int8 / fp8 / fp16).
 
-    ``wire = cast(grad * qmax / absmax)``; the fp32 ``inv = absmax / qmax`` travels with the
-    message and ``decode = wire * inv``.
+    ``wire = cast(grad / inv)`` with the fp32 ``inv = absmax / qmax``, which travels with the message;
+    ``decode = wire * inv``.  ``absmax`` is the largest ``|g|`` over the FINITE elements (1 if none is non-zero), so
+    an Inf element saturates to +-qmax, decodes to +-absmax and leaves the rest of the tensor its resolution.  The
+    cast rounds to nearest even and saturates at +-qmax; NaN stays NaN (int8: the code -128, which decodes to NaN).
     """
 
     def __init__(self, dtype="int8"):
@@ -208,8 +219,8 @@ class Scale(Coding):
     def encode(self, grad, **kwargs):
         g = grad.detach().float()
         qmax = _WIRE_MAX[self.wire]
-        amax = g.abs().max() if g.numel() else g.new_zeros(())
-        amax = torch.where(torch.isfinite(amax) & (amax > 0), amax, torch.ones_like(amax))
+        amax = torch.where(torch.isfinite(g), g.abs(), g.new_zeros(())).max() if g.numel() else g.new_zeros(())
+        amax = torch.where(amax > 0, amax, torch.ones_like(amax))
         inv = amax / torch.full_like(amax, qmax)   # IEEE fp32 division (a Python-scalar divisor is a
         #                                            reciprocal-multiply on CUDA and differs by 1 ulp)
         q = _sat_cast(g / inv, self.wire)       # == g * (qmax/amax) up to fp32 rounding
@@ -218,7 +229,10 @@ class Scale(Coding):
     def decode(self, code, cuda=False):
         q = self._place(_as_tensor(code["q"]), cuda)
         inv = self._place(_as_tensor(code["inv"]), cuda).float()
-        return q.float() * inv
+        f = q.float()
+        if q.dtype == torch.int8:
+            f = torch.where(q == -128, torch.full_like(f, float("nan")), f)
+        return f * inv
 
     def device_spec(self):
         return DeviceCodeSpec(KIND_SCALED, self.wire)

@@ -206,16 +206,21 @@ __device__ __forceinline__ void unpack_i8x8(const uint2& v, float* f) {
 #pragma unroll
   for (int i = 0; i < 2; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) f[4 * i + j] = (float)(int8_t)((w[i] >> (8 * j)) & 0xffu);
+    for (int j = 0; j < 4; ++j) {
+      const int8_t c = (int8_t)((w[i] >> (8 * j)) & 0xffu);
+      f[4 * i + j] = c == -128 ? __uint_as_float(0x7fffffffu) : (float)c;   // -128 is the NaN code (pack_i8x4)
+    }
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
 }
+// Narrowing to fp16 (cvt.rn.satfinite): round to nearest even, finite values and +-Inf saturate at +-65504, NaN stays NaN
+// (fmaxf / fminf would turn it into the other operand; the NaN test is on the bits, so no math-mode flag can drop it).
 __device__ __forceinline__ uint32_t pack_f16x2_sat(float a, float b) {
-  a = fminf(fmaxf(a, -65504.f), 65504.f);
-  b = fminf(fmaxf(b, -65504.f), 65504.f);
+  a = (__float_as_uint(a) & 0x7fffffffu) > 0x7f800000u ? a : fminf(fmaxf(a, -65504.f), 65504.f);
+  b = (__float_as_uint(b) & 0x7fffffffu) > 0x7f800000u ? b : fminf(fmaxf(b, -65504.f), 65504.f);
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
 }
@@ -230,10 +235,12 @@ __device__ __forceinline__ uint32_t pack_fp8x4(float a, float b, float c, float 
   uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c, d), __NV_SATFINITE, k);
   return lo | (hi << 16);
 }
+// int8 wire: clamp to +-127 (+-Inf included), round to nearest even; NaN is written as -128, which the clamp never produces.
+// The clamp comes first, so the conversion only ever sees values in range.
 __device__ __forceinline__ uint32_t pack_i8x4(float a, float b, float c, float d) {
   auto q = [](float x) -> uint32_t {
-    int v = __float2int_rn(x);
-    v = max(-127, min(127, v));
+    if ((__float_as_uint(x) & 0x7fffffffu) > 0x7f800000u) return 0x80u;
+    const int v = __float2int_rn(fminf(fmaxf(x, -127.f), 127.f));
     return (uint32_t)(uint8_t)(int8_t)v;
   };
   return q(a) | (q(b) << 8) | (q(c) << 16) | (q(d) << 24);

@@ -92,7 +92,7 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_absmax_kernel(const __grid_co
   load_grad8(a, entry, ti, tile, g);
   float m = 0.f;
 #pragma unroll
-  for (int j = 0; j < PSB_EPT; ++j) m = fmaxf(m, fabsf(g[j]));   // NaN-ignoring, like a finite-only max
+  for (int j = 0; j < PSB_EPT; ++j) m = fmaxf(m, isfinite(g[j]) ? fabsf(g[j]) : 0.f);   // amax over finite elements only
   m = block_max(m, red);
   if (threadIdx.x == 0) atomicMax(a.amax_bits + ti.param, __float_as_uint(m));
 }
@@ -100,8 +100,9 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_absmax_kernel(const __grid_co
 // ------------------------------------------------------------------------------------------
 // encode: gradient tile → wire tile (dense cast | abs-max scaled | block-wise top-k)
 // ------------------------------------------------------------------------------------------
+// `saturate` = false only when the fp16 wire carries an fp16 gradient: then it is an exact copy, +-Inf included.
 template <int WIRE>
-__device__ __forceinline__ void store_dense(void* wire_tile, const float* q) {
+__device__ __forceinline__ void store_dense(void* wire_tile, const float* q, bool saturate) {
   const int tid = threadIdx.x;
   if constexpr (WIRE == WIRE_F32) {
     uint4* p = reinterpret_cast<uint4*>(reinterpret_cast<float*>(wire_tile) + tid * PSB_EPT);
@@ -112,8 +113,9 @@ __device__ __forceinline__ void store_dense(void* wire_tile, const float* q) {
           make_uint4(pack_bf16x2(q[0], q[1]), pack_bf16x2(q[2], q[3]), pack_bf16x2(q[4], q[5]), pack_bf16x2(q[6], q[7])));
   } else if constexpr (WIRE == WIRE_F16) {
     st_v4(reinterpret_cast<uint16_t*>(wire_tile) + tid * PSB_EPT,
-          make_uint4(pack_f16x2_sat(q[0], q[1]), pack_f16x2_sat(q[2], q[3]), pack_f16x2_sat(q[4], q[5]),
-                     pack_f16x2_sat(q[6], q[7])));
+          saturate ? make_uint4(pack_f16x2_sat(q[0], q[1]), pack_f16x2_sat(q[2], q[3]), pack_f16x2_sat(q[4], q[5]),
+                                pack_f16x2_sat(q[6], q[7]))
+                   : make_uint4(pack_f16x2(q[0], q[1]), pack_f16x2(q[2], q[3]), pack_f16x2(q[4], q[5]), pack_f16x2(q[6], q[7])));
   } else if constexpr (WIRE == WIRE_E4M3 || WIRE == WIRE_E5M2) {
     uint2 v = make_uint2(pack_fp8x4<WIRE>(q[0], q[1], q[2], q[3]), pack_fp8x4<WIRE>(q[4], q[5], q[6], q[7]));
     *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(wire_tile) + tid * PSB_EPT) = v;
@@ -134,7 +136,7 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_co
   load_grad8(a, entry, ti, tile, g);
 
   if constexpr (KIND == KIND_DENSE) {
-    store_dense<WIRE>(wire_tile, g);
+    store_dense<WIRE>(wire_tile, g, a.grad_dt != DT_F16);
   } else if constexpr (KIND == KIND_SCALED) {
     float amax = __uint_as_float(a.amax_bits[ti.param]);
     if (!(amax > 0.f) || !isfinite(amax)) amax = 1.f;
@@ -143,7 +145,7 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_co
     float q[PSB_EPT];
 #pragma unroll
     for (int j = 0; j < PSB_EPT; ++j) q[j] = __fdiv_rn(g[j], inv);
-    store_dense<WIRE>(wire_tile, q);
+    store_dense<WIRE>(wire_tile, q, true);
   } else {  // KIND_TOPK: block-wise magnitude top-k, ties → lower index, entries in index order
     __shared__ uint32_t hist[256];
     __shared__ uint32_t warp_tot[PSB_THREADS / 32];

@@ -166,7 +166,13 @@ static inline unsigned __float_as_uint(float f) { unsigned u; memcpy(&u, &f, 4);
 static inline float __uint_as_float(unsigned u) { float f; memcpy(&f, &u, 4); return f; }
 static inline float __fdiv_rn(float a, float b) { return a / b; }
 static inline float __fsqrt_rn(float a) { return sqrtf(a); }
-static inline int __float2int_rn(float a) { return (int)nearbyintf(a); }
+// cvt.rni.s32.f32: round to nearest even; NaN gives 0 and out-of-range values (+-Inf included) saturate
+static inline int __float2int_rn(float a) {
+  if (std::isnan(a)) return 0;
+  if (a >= 2147483648.f) return 2147483647;
+  if (a <= -2147483648.f) return -2147483647 - 1;
+  return (int)nearbyintf(a);
+}
 
 #include "common.cuh"      // constants, TileInfo, GroupHyper, wire_elem_bytes (host part of the real header)
 
