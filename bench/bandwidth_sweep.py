@@ -38,6 +38,22 @@ import pytorch_ps_mpi_b200 as ps   # noqa: E402
 NVLINK_DATASHEET_GBS = 450.0    # H100 SXM NVLink 4, per direction per GPU (data sheet); --peer-copy measures it instead
 
 
+def code_of(arg: str):
+    """``--code``: identity | cast:<dtype> | scale:<dtype> | topk:<ratio> | qsgd:<levels> (block-wise QSGD)."""
+    kind, _, val = arg.partition(":")
+    if kind == "identity":
+        return ps.Identity()
+    if kind == "topk":
+        return ps.TopK(ratio=float(val), values="bf16")
+    if kind == "qsgd":
+        return ps.QSGD(levels=int(val), blockwise=True)
+    if kind == "scale":
+        return ps.Scale(val)
+    if kind == "cast":
+        return ps.Cast(val)
+    raise ValueError(f"unknown --code {arg!r}")
+
+
 def timed(w, device, fn, iters, warm=3):
     for _ in range(warm):
         fn()
@@ -128,9 +144,7 @@ def main():
             opt = eng = None
             wire = n * esz
             if impl == "fused":
-                code = ps.Identity() if a.code == "identity" else (
-                    ps.TopK(ratio=float(a.code.split(":")[1]), values="bf16") if a.code.startswith("topk") else
-                    ps.Cast(a.code.split(":")[1]))
+                code = code_of(a.code)
                 named = [(f"v{i}", p) for i, p in enumerate(params)]
                 opt = ps.SGD(named, params, lr=1e-3, code=code, mode="ps", engine="device", reduce=a.reduce, cuda=True)
                 eng = opt._engine

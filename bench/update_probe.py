@@ -15,7 +15,9 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import pytorch_ps_mpi_b200 as ps   # noqa: E402
+from bandwidth_sweep import code_of   # noqa: E402
 
 
 def main():
@@ -33,7 +35,7 @@ def main():
     shapes = [piece] * (n // piece) + ([n % piece] if n % piece else [])
     params = [torch.nn.Parameter(torch.zeros(m, device=dev, dtype=torch.bfloat16)) for m in shapes]
     grads = [torch.randn(m, device=dev).bfloat16() for m in shapes]
-    code = ps.Identity() if a.code == "identity" else ps.TopK(ratio=float(a.code.split(":")[1]), values="bf16")
+    code = code_of(a.code)
     opt = ps.SGD([(f"v{i}", p) for i, p in enumerate(params)], params, lr=1e-3, momentum=0.9, code=code, mode="ps",
                  engine="device", reduce=a.reduce)
     eng = opt._engine

@@ -22,25 +22,27 @@ Arbitrary user codings (any object with ``encode``/``decode``) keep working on t
 from __future__ import annotations
 
 import math
+import zlib
 from dataclasses import dataclass
 from typing import Any, List, Optional
 
+import numpy as np
 import torch
 
 __all__ = [
     "Coding", "Identity", "Cast", "Scale", "TopK", "QSGD", "SVD", "DeviceCodeSpec", "TILE",
-    "WIRE_F32", "WIRE_BF16", "WIRE_F16", "WIRE_E4M3", "WIRE_E5M2", "WIRE_I8",
-    "KIND_DENSE", "KIND_SCALED", "KIND_TOPK", "wire_dtype_of", "wire_code_of", "tile_k",
+    "WIRE_F32", "WIRE_BF16", "WIRE_F16", "WIRE_E4M3", "WIRE_E5M2", "WIRE_I8", "WIRE_I4",
+    "KIND_DENSE", "KIND_SCALED", "KIND_TOPK", "KIND_QSGD", "wire_dtype_of", "wire_code_of", "tile_k", "philox4x32_10",
 ]
 
 #: elements per tile of the flat arena; every parameter starts on a tile boundary and the
 #: block-wise top-k selects inside one tile.  Must match ``PSB_TILE`` in csrc/kernels/common.cuh.
 TILE = 2048
 
-# wire element types (must match csrc/kernels/common.cuh)
-WIRE_F32, WIRE_BF16, WIRE_F16, WIRE_E4M3, WIRE_E5M2, WIRE_I8 = 0, 1, 2, 3, 4, 5
+# wire element types (must match csrc/kernels/common.cuh); WIRE_I4 = two 4-bit codes per byte (block-wise QSGD only)
+WIRE_F32, WIRE_BF16, WIRE_F16, WIRE_E4M3, WIRE_E5M2, WIRE_I8, WIRE_I4 = 0, 1, 2, 3, 4, 5, 6
 # coding kinds
-KIND_DENSE, KIND_SCALED, KIND_TOPK = 0, 1, 2
+KIND_DENSE, KIND_SCALED, KIND_TOPK, KIND_QSGD = 0, 1, 2, 3
 
 _WIRE_TORCH = {
     WIRE_F32: torch.float32, WIRE_BF16: torch.bfloat16, WIRE_F16: torch.float16,
@@ -82,10 +84,12 @@ def tile_k(ratio: float, valid: int) -> int:
 class DeviceCodeSpec:
     """Fixed binary wire layout of a built-in coding (consumed by the CUDA kernels)."""
 
-    kind: int                 # KIND_DENSE | KIND_SCALED | KIND_TOPK
+    kind: int                 # KIND_DENSE | KIND_SCALED | KIND_TOPK | KIND_QSGD
     wire: int                 # WIRE_* element type of the payload values (-1 = same as grad)
     ratio: float = 1.0        # top-k keep ratio (KIND_TOPK)
     error_feedback: bool = False
+    levels: int = 0           # largest code magnitude (KIND_QSGD)
+    seed: int = 0             # Philox key (KIND_QSGD)
 
     def resolved_wire(self, grad_dtype: torch.dtype) -> int:
         return wire_code_of(grad_dtype) if self.wire < 0 else self.wire
@@ -95,6 +99,9 @@ class DeviceCodeSpec:
         return tile_k(self.ratio, TILE) if self.kind == KIND_TOPK else TILE
 
     def bytes_per_tile(self, grad_dtype: torch.dtype) -> int:
+        if self.kind == KIND_QSGD:
+            # 2048 codes (int8, or int4 two per byte) + a 16-byte header: fp32 scale, 12 zero bytes
+            return (TILE if self.wire == WIRE_I8 else TILE // 2) + 16
         w = self.resolved_wire(grad_dtype)
         esz = torch.empty((), dtype=_WIRE_TORCH[w]).element_size()
         if self.kind == KIND_TOPK:
@@ -337,20 +344,146 @@ class TopK(Coding):
         return f"TopK({what}, values={_WIRE_TORCH[self.wire]}, exact={self.exact})"
 
 
+_PHILOX_M0, _PHILOX_M1, _PHILOX_W0, _PHILOX_W1 = 0xD2511F53, 0xCD9E8D57, 0x9E3779B9, 0xBB67AE85
+_U32 = 0xFFFFFFFF
+
+
+def philox4x32_10(c0, c1, c2, c3, k0, k1):
+    """Philox4x32-10 (Random123): counter words ``c0..c3`` and key words ``k0, k1`` (integers or numpy arrays) → the four
+    output words as uint64 numpy arrays holding 32-bit values.  Same rounds as ``psb::philox4x32_10`` in common.cuh."""
+    c = [np.asarray(x, np.uint64) & np.uint64(_U32) for x in (c0, c1, c2, c3)]
+    k0, k1 = (np.asarray(x, np.uint64) & np.uint64(_U32) for x in (k0, k1))
+    m, sh = np.uint64(_U32), np.uint64(32)
+    for _ in range(10):
+        p0, p1 = np.uint64(_PHILOX_M0) * c[0], np.uint64(_PHILOX_M1) * c[2]
+        c = [(p1 >> sh) ^ c[1] ^ k0, p1 & m, (p0 >> sh) ^ c[3] ^ k1, p0 & m]
+        k0, k1 = (k0 + np.uint64(_PHILOX_W0)) & m, (k1 + np.uint64(_PHILOX_W1)) & m
+    return c
+
+
 class QSGD(Coding):
     """QSGD-style stochastic quantisation (Alistarh et al. 2017): ``sign · ‖g‖₂ · ξ/levels`` with ``ξ`` drawn so
-    the code is an unbiased estimate of the gradient.  Host (generic-object) path — the kind of user coding the
-    reference's external ``codings`` module carried (SURVEY §2.2); the fused device codings are
-    :class:`Cast` / :class:`Scale` / :class:`TopK`.
+    the code is an unbiased estimate of the gradient.
+
+    ``blockwise=False`` (default): whole-tensor norm, int8 / int16 codes, host (generic-object) path only — the kind of user
+    coding the reference's external ``codings`` module carried (SURVEY §2.2).
+
+    ``blockwise=True``: every ``TILE``-element block of the flattened tensor is quantised against its own L2 norm, fused into the
+    device engine's encode and update kernels.  ``levels`` in [1, 127]; ``levels <= 7`` travels as 4-bit two's-complement codes,
+    two per byte (element ``2i`` in the low nibble, -8 = NaN), otherwise as int8 codes (-128 = NaN).  A wire tile is the 2048
+    codes followed by a 16-byte header: the fp32 ``scale = norm / levels`` and 12 zero bytes (1040 or 2064 bytes per tile).
+    The rules (DESIGN.md, wire numerics): ``norm`` is the L2 norm of the tile's finite elements (1 if none is non-zero),
+    ``x = |g| / norm · levels``, ``q = sign(g) · (floor(x) + [u < x − floor(x)])``, ±Inf saturates to ±levels, NaN gets the NaN
+    code, and ``u`` is word ``e & 3`` of Philox4x32-10 with counter ``(e >> 2, arena tile, step, rank)`` and key ``seed``
+    (``None`` = 0), ``e`` the element's index in its tile.  ``decode`` returns ``q · scale``, so ``E[decode] == g``.
+
+    :meth:`encode` is the kernels' oracle and the host engine's path; it returns ``{"wire": uint8 [ntiles, bytes_per_tile],
+    "shape": ...}``, the exact bytes the device writes.  The device engine passes the arena tile, its step counter and the
+    rank.  The host engine passes only ``name=``; then ``step`` is the number of earlier ``encode`` calls for that name in
+    this object, ``rank`` the process rank of the initialised runtime (0 without one), and the first tile
+    ``zlib.crc32(name)``, so that ranks, steps and parameters draw independent numbers.
     """
 
-    def __init__(self, levels: int = 255, seed: Optional[int] = None):
+    def __init__(self, levels: int = 255, seed: Optional[int] = None, blockwise: bool = False):
+        self.blockwise = bool(blockwise)
+        if self.blockwise:
+            if not 1 <= levels <= 127:
+                raise ValueError("QSGD(blockwise=True) needs levels in [1, 127]")
+            self.levels = int(levels)
+            self.seed = 0 if seed is None else int(seed) & ((1 << 64) - 1)
+            self.wire = WIRE_I4 if self.levels <= 7 else WIRE_I8
+            self._calls = {}
+            return
         if not 1 <= levels <= 32767:
             raise ValueError("levels must be in [1, 32767]")
         self.levels = int(levels)
         self._gen = torch.Generator().manual_seed(seed) if seed is not None else None
 
-    def encode(self, grad, **kwargs):
+    def device_spec(self):
+        if not self.blockwise:
+            return None
+        return DeviceCodeSpec(KIND_QSGD, self.wire, levels=self.levels, seed=self.seed)
+
+    def _encode_blockwise(self, grad, name, step, rank, first_tile):
+        if step is None:
+            step = self._calls.get(name, 0)
+            self._calls[name] = step + 1
+        if rank is None:
+            from . import runtime
+            rank = runtime.rank() if runtime.is_initialized() else 0
+        if first_tile is None:
+            first_tile = zlib.crc32(name.encode()) if name is not None else 0
+        flat = grad.detach().reshape(-1).float().cpu()
+        n = flat.numel()
+        nt = max(1, (n + TILE - 1) // TILE)
+        g = torch.zeros(nt * TILE, dtype=torch.float32)
+        g[:n] = flat
+        g = g.view(nt, TILE)
+        fin = torch.isfinite(g)
+        a = torch.where(fin, g.abs(), torch.zeros_like(g))
+        m = a.max(dim=1).values
+        any_ = m > 0
+        m = torch.where(any_, m, torch.ones_like(m))
+        t = torch.where(fin, a / m[:, None], torch.zeros_like(g))
+        # fp32 sum of t² in the kernel's order: 8 elements per thread in index order, xor butterfly over 32 lanes, 8 warps in order
+        sq = (t * t).view(nt, 256, 8)
+        s = sq[:, :, 0].clone()
+        for j in range(1, 8):
+            s = s + sq[:, :, j]
+        s = s.view(nt, 8, 32)
+        lane = torch.arange(32)
+        for off in (16, 8, 4, 2, 1):
+            s = s + s[:, :, lane ^ off]
+        tot = s[:, 0, 0].clone()
+        for w in range(1, 8):
+            tot = tot + s[:, w, 0]
+        # correctly rounded fp32 sqrt (= __fsqrt_rn): via float64, since torch's vectorised fp32 sqrt may be 1 ulp off
+        r = torch.where(any_, torch.sqrt(tot.double()).float(), torch.ones_like(tot))
+        lv = torch.tensor(float(self.levels), dtype=torch.float32)
+        x = (t / r[:, None]) * lv
+        fl = torch.floor(x)
+        e = np.arange(TILE)
+        tiles = (np.arange(nt, dtype=np.uint64) + np.uint64(first_tile))[:, None]
+        words = philox4x32_10(e[None, :] >> 2, tiles, step, rank, self.seed & _U32, self.seed >> 32)
+        w = np.choose(e & 3, words).astype(np.int64)                      # word e & 3 of the element's draw
+        u = torch.from_numpy(w >> 8).float() * 2.0 ** -24
+        qi = torch.clamp(fl.long() + (u < x - fl).long(), max=self.levels)
+        qi = torch.where(torch.isinf(g), torch.full_like(qi, self.levels), qi)
+        q = torch.where(torch.signbit(g), -qi, qi)
+        nan_code, mask = (-8, 0xF) if self.wire == WIRE_I4 else (-128, 0xFF)
+        q = torch.where(torch.isnan(g), torch.full_like(q, nan_code), q) & mask
+        if self.wire == WIRE_I4:
+            payload = (q[:, 0::2] | (q[:, 1::2] << 4)).to(torch.uint8)
+        else:
+            payload = q.to(torch.uint8)
+        scale = m * (r / lv)
+        fmax = torch.finfo(torch.float32).max
+        scale = torch.where(scale > fmax, torch.full_like(scale, fmax), scale)
+        header = torch.zeros(nt, 4, dtype=torch.float32)
+        header[:, 0] = scale
+        wire = torch.cat([payload, header.view(torch.uint8)], dim=1)
+        return {"wire": wire, "shape": tuple(grad.shape), "levels": self.levels}
+
+    def _decode_blockwise(self, code, cuda):
+        wire = _as_tensor(code["wire"]).cpu()
+        shape = tuple(int(d) for d in code["shape"])
+        pay = wire.shape[1] - 16
+        scale = wire[:, pay: pay + 4].contiguous().view(torch.float32)
+        if pay == TILE // 2:
+            b = wire[:, :pay].to(torch.int32)
+            q = torch.stack([b & 0xF, b >> 4], dim=2).reshape(wire.shape[0], TILE)
+            q = q - ((q & 0x8) << 1)                                          # sign-extend the nibbles
+            nan = q == -8
+        else:
+            q = wire[:, :pay].contiguous().view(torch.int8).to(torch.int32)
+            nan = q == -128
+        f = torch.where(nan, torch.full(q.shape, float("nan")), q.float()) * scale
+        n = math.prod(shape)
+        return self._place(f.reshape(-1)[:n].reshape(shape), cuda)
+
+    def encode(self, grad, name=None, step=None, rank=None, first_tile=None, **kwargs):
+        if self.blockwise:
+            return self._encode_blockwise(grad, name, step, rank, first_tile)
         g = grad.detach().float().cpu()
         norm = g.norm()
         if float(norm) == 0.0 or not torch.isfinite(norm):
@@ -364,11 +497,15 @@ class QSGD(Coding):
         return {"q": q.to(dt), "norm": norm.reshape(1), "levels": self.levels, "shape": tuple(g.shape)}
 
     def decode(self, code, cuda=False):
+        if "wire" in code:
+            return self._decode_blockwise(code, cuda)
         q = self._place(_as_tensor(code["q"]), cuda).float()
         norm = self._place(_as_tensor(code["norm"]), cuda).float()
         return (q * (norm / float(code["levels"]))).reshape(tuple(int(d) for d in code["shape"]))
 
     def __repr__(self):
+        if self.blockwise:
+            return f"QSGD(levels={self.levels}, blockwise=True)"
         return f"QSGD(levels={self.levels})"
 
 

@@ -21,9 +21,9 @@
 #define PSB_MAX_GROUPS 16
 
 // wire element types (codings.py WIRE_*)
-enum : int { WIRE_F32 = 0, WIRE_BF16 = 1, WIRE_F16 = 2, WIRE_E4M3 = 3, WIRE_E5M2 = 4, WIRE_I8 = 5 };
+enum : int { WIRE_F32 = 0, WIRE_BF16 = 1, WIRE_F16 = 2, WIRE_E4M3 = 3, WIRE_E5M2 = 4, WIRE_I8 = 5, WIRE_I4 = 6 };
 // coding kinds (codings.py KIND_*)
-enum : int { KIND_DENSE = 0, KIND_SCALED = 1, KIND_TOPK = 2 };
+enum : int { KIND_DENSE = 0, KIND_SCALED = 1, KIND_TOPK = 2, KIND_QSGD = 3 };
 // parameter / gradient dtypes
 enum : int { DT_F32 = 0, DT_BF16 = 1, DT_F16 = 2 };
 // optimizers
@@ -288,6 +288,49 @@ PSB_HD constexpr int wire_elem_bytes(int wire) {
 }
 PSB_HD constexpr float wire_qmax(int wire) {
   return wire == WIRE_E4M3 ? 448.f : wire == WIRE_E5M2 ? 57344.f : wire == WIRE_I8 ? 127.f : 65504.f;
+}
+
+// fp32 multiply / add rounded to nearest even and never contracted into an FMA: the explicit-rounding intrinsics on the
+// device; on the host (a plain-C++ build of the kernels, e.g. their CPU emulation) ordinary IEEE arithmetic.
+PSB_HD inline float mul_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+PSB_HD inline float add_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+// 4-byte load coherent at system scope (a peer's memory over NVLink); on the host a plain load.
+PSB_HD inline uint32_t ld_sys_u32(const void* p) {
+#ifdef __CUDA_ARCH__
+  uint32_t v;
+  asm volatile("ld.relaxed.sys.global.L1::no_allocate.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+#else
+  return *static_cast<const uint32_t*>(p);
+#endif
+}
+
+// Philox4x32-10 (Salmon et al., SC'11; the generator of Random123 and curand): counter c, key k → four uniform 32-bit words.
+// Plain integer code (64-bit products rather than __umulhi), so the host, the CPU emulator and numpy reproduce it bit for bit.
+struct Philox4 {
+  uint32_t w[4];
+};
+PSB_HD inline Philox4 philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint64_t p0 = (uint64_t)0xD2511F53u * c0, p1 = (uint64_t)0xCD9E8D57u * c2;
+    const uint32_t n0 = (uint32_t)(p1 >> 32) ^ c1 ^ k0, n2 = (uint32_t)(p0 >> 32) ^ c3 ^ k1;
+    c1 = (uint32_t)p1, c3 = (uint32_t)p0, c0 = n0, c2 = n2;
+    k0 += 0x9E3779B9u, k1 += 0xBB67AE85u;
+  }
+  return Philox4{{c0, c1, c2, c3}};
 }
 
 }  // namespace psb

@@ -34,6 +34,11 @@ struct EncodeArgs {
   int32_t sig_slot;
   uint64_t sig_value;
   unsigned int* sig_counter;   // zero before launch; left zero
+  // KIND_QSGD: Philox key = seed, counter = (element/4, arena tile, step, rank); levels = the largest code magnitude
+  uint64_t seed;
+  uint32_t step;
+  uint32_t rank;
+  int32_t levels;
 };
 
 struct UpdateArgs {

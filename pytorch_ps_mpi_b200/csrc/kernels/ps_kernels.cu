@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_absmax_kernel(const __grid_co
 }
 
 // ------------------------------------------------------------------------------------------
-// encode: gradient tile → wire tile (dense cast | abs-max scaled | block-wise top-k)
+// encode: gradient tile → wire tile (dense cast | abs-max scaled | block-wise top-k | block-wise QSGD)
 // ------------------------------------------------------------------------------------------
 // `saturate` = false only when the fp16 wire carries an fp16 gradient: then it is an exact copy, +-Inf included.
 template <int WIRE>
@@ -125,6 +125,92 @@ __device__ __forceinline__ void store_dense(void* wire_tile, const float* q, boo
   }
 }
 
+// Block-wise QSGD (KIND_QSGD): one wire tile = the 2048 codes (int8, or int4 two per byte with element 2i in the low nibble),
+// then a 16-byte header holding the fp32 scale and 12 zero bytes.  The rules are those of DESIGN.md (wire numerics); every
+// float operation is an explicit round-to-nearest (mul_rn / add_rn / __fdiv_rn / __fsqrt_rn), so no FMA contraction changes a
+// bit and a host build of this code (the CPU emulator) computes the same codes.
+template <int WIRE>
+constexpr int qsgd_payload_bytes() {
+  return WIRE == WIRE_I4 ? PSB_TILE / 2 : PSB_TILE;
+}
+
+template <int WIRE>
+__device__ __forceinline__ void qsgd_encode_tile(const EncodeArgs& a, int tile, uint8_t* wire_tile, const float* g) {
+  __shared__ float red[PSB_THREADS / 32];
+  const int tid = threadIdx.x;
+  // norm = m * r: m = abs-max over the finite elements (exact, so its reduction order is free), r = sqrt(sum of (|g| / m)^2) —
+  // the tile scaled by m first, so no finite input overflows; sum order: per thread in index order, xor butterfly, warps in order
+  float m = 0.f;
+#pragma unroll
+  for (int j = 0; j < PSB_EPT; ++j) m = fmaxf(m, isfinite(g[j]) ? fabsf(g[j]) : 0.f);
+  m = block_max(m, red);
+  const bool any = m > 0.f;
+  if (!any) m = 1.f;
+  float t[PSB_EPT], s = 0.f;
+#pragma unroll
+  for (int j = 0; j < PSB_EPT; ++j) {
+    t[j] = isfinite(g[j]) ? __fdiv_rn(fabsf(g[j]), m) : 0.f;
+    s = add_rn(s, mul_rn(t[j], t[j]));
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) s = add_rn(s, __shfl_xor_sync(0xffffffffu, s, off));
+  if ((tid & 31) == 0) red[tid >> 5] = s;
+  __syncthreads();
+  s = red[0];
+#pragma unroll
+  for (int w = 1; w < PSB_THREADS / 32; ++w) s = add_rn(s, red[w]);
+  const float r = any ? __fsqrt_rn(s) : 1.f;   // >= 1 when any: the abs-max element contributes exactly 1
+  const int levels = a.levels;
+  const float lv = (float)levels;
+
+  // q = sign(g) * (floor(x) + [u < x - floor(x)]), x = |g| / m / r * levels; u = (Philox word >> 8) * 2^-24
+  const uint32_t k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32);
+  const Philox4 ra = philox4x32_10(2 * tid, (uint32_t)tile, a.step, a.rank, k0, k1);
+  const Philox4 rb = philox4x32_10(2 * tid + 1, (uint32_t)tile, a.step, a.rank, k0, k1);
+  constexpr uint32_t NAN_CODE = WIRE == WIRE_I4 ? 0x8u : 0x80u;
+  constexpr uint32_t MASK = WIRE == WIRE_I4 ? 0xfu : 0xffu;
+  uint32_t code[PSB_EPT];
+#pragma unroll
+  for (int j = 0; j < PSB_EPT; ++j) {
+    const uint32_t w = j < 4 ? ra.w[j] : rb.w[j - 4];
+    const float u = mul_rn((float)(w >> 8), 5.9604644775390625e-8f);   // 2^-24
+    int qi;
+    if (!isfinite(g[j])) {
+      qi = levels;                                                          // +-Inf saturates (NaN: replaced below)
+    } else {
+      const float x = mul_rn(__fdiv_rn(t[j], r), lv);
+      const float fl = floorf(x);
+      qi = min((int)fl + (u < add_rn(x, -fl) ? 1 : 0), levels);
+    }
+    const int q = (__float_as_uint(g[j]) >> 31) ? -qi : qi;
+    code[j] = (__float_as_uint(g[j]) & 0x7fffffffu) > 0x7f800000u ? NAN_CODE : (uint32_t)q & MASK;
+  }
+  if constexpr (WIRE == WIRE_I4) {
+    uint32_t v = 0;
+#pragma unroll
+    for (int j = 0; j < PSB_EPT; ++j) v |= code[j] << (4 * j);
+    *reinterpret_cast<uint32_t*>(wire_tile + tid * 4) = v;
+  } else {
+    const uint2 v = make_uint2(code[0] | code[1] << 8 | code[2] << 16 | code[3] << 24,
+                               code[4] | code[5] << 8 | code[6] << 16 | code[7] << 24);
+    *reinterpret_cast<uint2*>(wire_tile + tid * 8) = v;
+  }
+  if (tid == 0) {
+    float scale = mul_rn(m, __fdiv_rn(r, lv));          // norm / levels, without the overflow of forming norm first
+    if (!(scale <= 3.40282346638528859811704183484516925e+38f)) scale = 3.40282346638528859811704183484516925e+38f;
+    st_v4(wire_tile + qsgd_payload_bytes<WIRE>(), make_uint4(__float_as_uint(scale), 0u, 0u, 0u));
+  }
+}
+
+// int4 wire: eight two's-complement nibbles, element j in bits [4j, 4j + 4); -8 is the NaN code
+__device__ __forceinline__ void unpack_i4x8(uint32_t w, float* f) {
+#pragma unroll
+  for (int j = 0; j < PSB_EPT; ++j) {
+    const int c = (int)(w << (28 - 4 * j)) >> 28;
+    f[j] = c == -8 ? __uint_as_float(0x7fffffffu) : (float)c;
+  }
+}
+
 template <int KIND, int WIRE>
 __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_constant__ EncodeArgs a) {
   int entry, tile;
@@ -146,6 +232,8 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_co
 #pragma unroll
     for (int j = 0; j < PSB_EPT; ++j) q[j] = __fdiv_rn(g[j], inv);
     store_dense<WIRE>(wire_tile, q, true);
+  } else if constexpr (KIND == KIND_QSGD) {
+    qsgd_encode_tile<WIRE>(a, tile, wire_tile, g);
   } else {  // KIND_TOPK: block-wise magnitude top-k, ties → lower index, entries in index order
     __shared__ uint32_t hist[256];
     __shared__ uint32_t warp_tot[PSB_THREADS / 32];
@@ -508,6 +596,48 @@ __global__ void __launch_bounds__(PSB_THREADS, 3) psb_update_kernel(const __grid
       __syncthreads();
       apply_and_publish<OPT>(a, ti, e0, inv_count, acc, w, m, v, vm);
     }
+  } else if constexpr (KIND == KIND_QSGD) {
+    // ---- block-wise QSGD over P2P: each rank's codes (8 bytes per thread on the int8 wire, 4 on the int4 wire) and the scale
+    // in that rank's tile header, up to CH ranks in flight; q * scale summed in rank order ----
+    constexpr int CH = 4;
+    constexpr int PAY = qsgd_payload_bytes<WIRE>();
+    for (int tile = a.tile_begin + blockIdx.x; tile < a.tile_end; tile += gridDim.x) {
+      const TileInfo ti = a.tiles[tile];
+      if (a.active != nullptr && a.active[ti.param] == 0) continue;
+      const size_t e0 = (size_t)tile * PSB_TILE + tid * PSB_EPT;
+      const size_t tile_off = (size_t)tile * a.bytes_per_tile;
+      float acc[PSB_EPT], w[PSB_EPT], m[PSB_EPT], v[PSB_EPT], vm[PSB_EPT];
+#pragma unroll
+      for (int j = 0; j < PSB_EPT; ++j) acc[j] = 0.f;
+      load_state<OPT>(a, ti, e0, w, m, v, vm);
+      for (int r0 = 0; r0 < a.world; r0 += CH) {
+        uint2 q[CH];
+        float sc[CH];
+#pragma unroll
+        for (int c = 0; c < CH; ++c) {
+          const int r = r0 + c;
+          sc[c] = 0.f;
+          if (r < a.world && (contrib >> r & 1u)) {
+            const uint8_t* p = reinterpret_cast<const uint8_t*>(a.wire[r]) + tile_off;
+            if constexpr (WIRE == WIRE_I4) q[c].x = ld_sys_u32(p + tid * 4);
+            else q[c] = ld_sys_v2(p + tid * 8);
+            sc[c] = ld_sys_f32(reinterpret_cast<const float*>(p + PAY));
+          }
+        }
+#pragma unroll
+        for (int c = 0; c < CH; ++c) {       // fixed rank order → deterministic fp32 sum
+          const int r = r0 + c;
+          if (r < a.world && (contrib >> r & 1u)) {
+            float f[PSB_EPT];
+            if constexpr (WIRE == WIRE_I4) unpack_i4x8(q[c].x, f);
+            else unpack_i8x8(q[c], f);
+#pragma unroll
+            for (int j = 0; j < PSB_EPT; ++j) acc[j] += f[j] * sc[c];
+          }
+        }
+      }
+      apply_and_publish<OPT>(a, ti, e0, inv_count, acc, w, m, v, vm);
+    }
   } else {
     constexpr bool NVLS_OK = KIND == KIND_DENSE && (WIRE == WIRE_F32 || WIRE == WIRE_BF16 || WIRE == WIRE_F16);
     if (NVLS_OK && a.reduce == REDUCE_NVLS) {
@@ -850,6 +980,7 @@ void psb_launch_encode(cudaStream_t s, int kind, int wire, const EncodeArgs& a) 
   ENC(KIND_DENSE, WIRE_F32) ENC(KIND_DENSE, WIRE_BF16) ENC(KIND_DENSE, WIRE_F16) ENC(KIND_DENSE, WIRE_E4M3)
   ENC(KIND_DENSE, WIRE_E5M2) ENC(KIND_SCALED, WIRE_I8) ENC(KIND_SCALED, WIRE_E4M3) ENC(KIND_SCALED, WIRE_E5M2)
   ENC(KIND_SCALED, WIRE_F16) ENC(KIND_TOPK, WIRE_F32) ENC(KIND_TOPK, WIRE_BF16)
+  ENC(KIND_QSGD, WIRE_I8) ENC(KIND_QSGD, WIRE_I4)
 #undef ENC
 }
 
@@ -863,6 +994,7 @@ void psb_launch_update(cudaStream_t s, int kind, int wire, int opt, const Update
   UPD(KIND_DENSE, WIRE_F32) UPD(KIND_DENSE, WIRE_BF16) UPD(KIND_DENSE, WIRE_F16) UPD(KIND_DENSE, WIRE_E4M3)
   UPD(KIND_DENSE, WIRE_E5M2) UPD(KIND_SCALED, WIRE_I8) UPD(KIND_SCALED, WIRE_E4M3) UPD(KIND_SCALED, WIRE_E5M2)
   UPD(KIND_SCALED, WIRE_F16) UPD(KIND_TOPK, WIRE_F32) UPD(KIND_TOPK, WIRE_BF16)
+  UPD(KIND_QSGD, WIRE_I8) UPD(KIND_QSGD, WIRE_I4)
 #undef UPD
 }
 

@@ -34,7 +34,7 @@ from typing import Dict, List, Optional
 import torch
 
 from .. import runtime
-from ..codings import KIND_DENSE, KIND_SCALED, KIND_TOPK, TILE, WIRE_BF16, WIRE_F16, WIRE_F32, wire_code_of
+from ..codings import KIND_DENSE, KIND_QSGD, KIND_SCALED, KIND_TOPK, TILE, WIRE_BF16, WIRE_F16, WIRE_F32, wire_code_of
 from ..ops import ext
 from ..utils.misc import CudaStepTimer
 from .layout import FlatLayout
@@ -238,6 +238,10 @@ class DeviceEngine:
         self._residual_ptr = self.residual.data_ptr() if self.residual is not None else 0
         self._sigctr_ptr = self.counters.data_ptr() + 8
         self._ratio = float(self.spec.ratio)
+        # block-wise QSGD: the Philox counter holds (element, arena tile, step, rank).  `_qsgd_step` counts the steps this rank
+        # has encoded; it is saved with the optimizer state ("qsgd_step") on every rank, so a resumed run draws what a straight
+        # run draws.
+        self._qsgd_step = 0
         self._sig_base = [p + self.off_signal for p in self.arena.ptrs]
         # ---- the pipeline chunks: contiguous runs of whole parameters in arena (= backward) order ----
         self._make_chunks()
@@ -362,9 +366,12 @@ class DeviceEngine:
                 st["master_param"] = self._like(self.master[sl], s.param)
 
     def sync_state_to_torch(self):
+        o = self.opt
+        if self.kind == KIND_QSGD:
+            for s in self.layout.slots:
+                o.state[s.param]["qsgd_step"] = self._qsgd_step
         if not self.is_server:
             return
-        o = self.opt
         for s in self.layout.slots:   # SGD too: the first-step momentum rule (ps.py:203-205) needs it on resume
             o.state[s.param]["step"] = self._param_steps[s.index] if self.mode != "async" else self._group_steps[s.group]
 
@@ -372,9 +379,14 @@ class DeviceEngine:
         """After ``load_state_dict``: copy loaded tensors back into the flat (fp32) state.
 
         ``original`` maps ``id(param)`` → the un-cast saved state of that parameter."""
+        o = self.opt
+        if self.kind == KIND_QSGD:
+            for s in self.layout.slots:
+                st = original.get(id(s.param), {}) if original is not None else o.state.get(s.param, {})
+                if "qsgd_step" in st:
+                    self._qsgd_step = int(st["qsgd_step"])
         if not self.is_server:
             return
-        o = self.opt
         with torch.no_grad():
             for s in self.layout.slots:
                 st = o.state.get(s.param, {})
@@ -510,12 +522,14 @@ class DeviceEngine:
         items, self._chunk_items[k] = self._chunk_items[k], []
         if items:
             grads = [g for _, g in items]
+            qsgd = dict(seed=self.spec.seed, step=self._qsgd_step & 0xFFFFFFFF, rank=self.rank,
+                        levels=self.spec.levels) if self.kind == KIND_QSGD else {}
             m.encode(self.kind, self.wire, grads, [s.first_tile for s, _ in items],
                      [s.ntiles for s, _ in items], [s.index for s, _ in items],
                      self._tiles_ptr, self._wire_ptr, self._scales_ptr, self._amax_ptr, self._residual_ptr,
                      self.bpt, self.cap, self._ratio,
                      *((sig[0], sig[1], sig[2], self._sigctr_ptr) if sig else ([], 0, 0, 0)),
-                     csh)
+                     csh, **qsgd)
             nb = (len(items) + 63) // 64
             self.launches += nb * (2 if self.kind == KIND_SCALED else 1)
             self._keep.extend(grads)
@@ -712,6 +726,7 @@ class DeviceEngine:
         data["packaged_bytes"] = wire_bytes / nfired
         data["engine"] = "device"
         self._epoch += 1
+        self._qsgd_step += 1
         if len(self._fired) != L.nparams:
             self._uniform_steps = False              # some parameter sat this step out: per-parameter counts diverge from now on
         for i in self._fired:
