@@ -111,7 +111,7 @@ struct UpdatePlan {
       a.tile_end = std::min(hi, b + win);
       const bool first = b == lo, last = a.tile_end == hi;
       a.wait_grads = first ? wait_grads_all : 0;
-      a.signal_mode = last ? signal_all : 0;
+      a.signal_mode = last ? signal_all : SIGNAL_NONE;
       a.ack_mask = last ? ack_all : 0;
       a.ack_last = last ? 1 : 0;
       psb_launch_update(pick_stream(stream), kind, wire, opt, a, std::min(grid, a.tile_end - a.tile_begin));
@@ -229,6 +229,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("SIG_GRAD_VERSION") = SIG_GRAD_VERSION;
   m.attr("MAX_RANKS") = PSB_MAX_RANKS;
   m.attr("MAX_GROUPS") = PSB_MAX_GROUPS;
+  // launch modes (common.cuh); the enums are anonymous, so pybind11 needs them as plain ints
+  m.attr("OPT_SGD") = (int)OPT_SGD;
+  m.attr("OPT_ADAM") = (int)OPT_ADAM;
+  m.attr("BCAST_LOCAL") = (int)BCAST_LOCAL;
+  m.attr("BCAST_UNICAST") = (int)BCAST_UNICAST;
+  m.attr("BCAST_MULTICAST") = (int)BCAST_MULTICAST;
+  m.attr("REDUCE_P2P") = (int)REDUCE_P2P;
+  m.attr("REDUCE_NVLS") = (int)REDUCE_NVLS;
+  m.attr("SIGNAL_NONE") = (int)SIGNAL_NONE;
+  m.attr("SIGNAL_PARAMS_READY") = (int)SIGNAL_PARAMS_READY;
+  m.attr("SIGNAL_CONSUMED") = (int)SIGNAL_CONSUMED;
 
   py::class_<psb::SymmBlock, std::shared_ptr<psb::SymmBlock>>(m, "SymmBlock")
       .def(py::init<int, int, int, size_t, const std::string&>(), py::arg("rank"), py::arg("world"), py::arg("device"),

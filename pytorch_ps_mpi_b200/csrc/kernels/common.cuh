@@ -32,6 +32,8 @@ enum : int { OPT_SGD = 0, OPT_ADAM = 1 };
 enum : int { BCAST_LOCAL = 0, BCAST_UNICAST = 1, BCAST_MULTICAST = 2 };
 // how the gradient tiles are gathered
 enum : int { REDUCE_P2P = 0, REDUCE_NVLS = 1 };
+// which flag the last CTA of an update launch raises on every rank
+enum : int { SIGNAL_NONE = 0, SIGNAL_PARAMS_READY = 1, SIGNAL_CONSUMED = 2 };
 
 // signal-pad slots (uint64 each); pad is PSB_SIGNAL_SLOTS * 8 bytes at the start of the block
 #define PSB_SIGNAL_SLOTS 512

@@ -72,7 +72,7 @@ struct UpdateArgs {
   int32_t tile_begin, tile_end;        // this launch covers arena tiles [tile_begin, tile_end) — one chunk of the
                                        // pipeline (or the whole arena)
   int32_t wait_grads;                  // spin on SIG_GRAD_READY of every contributor first
-  int32_t signal_mode;                 // 0 none | 1 SIG_PARAMS_READY → all | 2 SIG_CONSUMED[rank] → all
+  int32_t signal_mode;                 // SIGNAL_NONE | SIGNAL_PARAMS_READY → all | SIGNAL_CONSUMED[rank] → all
   uint32_t ack_mask;                   // async: ranks to acknowledge (SIG_ACK) when done
   int32_t ack_last;                    // 1 on the last window of a launch sequence: the async contributors (chosen on the
                                        // device, select_out) are acknowledged only then

@@ -727,7 +727,7 @@ __global__ void __launch_bounds__(PSB_THREADS, 3) psb_update_kernel(const __grid
   // fence + completion atomic cost each CTA a round trip its warps wait out at the barrier (ncu: `barrier` was the top
   // stall of a 2-3-tile chunk launch).  Their stores are ordered before the last chunk's flag by the stream: a kernel's
   // writes — peer and multimem stores included — are complete when the kernel is.
-  if (a.signal_mode == 0 && ack == 0u) return;
+  if (a.signal_mode == SIGNAL_NONE && ack == 0u) return;
   __syncthreads();
   if (tid == 0) {
     __threadfence_system();
@@ -742,10 +742,10 @@ __global__ void __launch_bounds__(PSB_THREADS, 3) psb_update_kernel(const __grid
     }
     __threadfence_system();
     if (tid < a.world) {
-      if (a.signal_mode == 1) {
+      if (a.signal_mode == SIGNAL_PARAMS_READY) {
         st_release_sys(a.signal_peer[tid] + SIG_VERSION, a.version);
         st_release_sys(a.signal_peer[tid] + SIG_PARAMS_READY, a.epoch);
-      } else if (a.signal_mode == 2) {
+      } else if (a.signal_mode == SIGNAL_CONSUMED) {
         st_release_sys(a.signal_peer[tid] + SIG_CONSUMED + a.rank, a.epoch);
       }
       if (ack >> tid & 1u) {

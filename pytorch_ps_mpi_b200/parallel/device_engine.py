@@ -42,23 +42,15 @@ from .symmetric import SymmetricArena
 
 _DT = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 _DONE_EPOCH = 1 << 62
+# launch modes of psb_update_kernel (must match csrc/kernels/common.cuh; the extension exports the same names)
+OPT_SGD, OPT_ADAM = 0, 1
+BCAST_LOCAL, BCAST_UNICAST, BCAST_MULTICAST = 0, 1, 2
+REDUCE_P2P, REDUCE_NVLS = 0, 1
+SIGNAL_NONE, SIGNAL_PARAMS_READY, SIGNAL_CONSUMED = 0, 1, 2
 
 
 def _align(n: int, a: int = 256) -> int:
     return (n + a - 1) // a * a
-
-
-def _dense(t: torch.Tensor) -> bool:
-    """True if ``t``'s strides describe a dense, non-overlapping permutation of its shape."""
-    if t.is_contiguous():
-        return True
-    dims = sorted(((st, sz) for st, sz in zip(t.stride(), t.shape) if sz > 1), key=lambda x: x[0])
-    expect = 1
-    for st, sz in dims:
-        if st != expect:
-            return False
-        expect *= sz
-    return True
 
 
 class DeviceEngine:
@@ -118,16 +110,9 @@ class DeviceEngine:
         with torch.no_grad():
             self.wire_arena.zero_()          # tile padding must be (and then stays) zero: see grad_out()
             self.param_arena.zero_()
-            for s in L.slots:
-                flat = self.param_arena[s.offset: s.offset + s.numel]
-                pd = s.param.data
-                if s.strides is not None:   # custom placement requested by the module (layout.py): padding stays zero
-                    view = torch.as_strided(flat, pd.shape, s.strides)
-                elif pd.is_contiguous() or not _dense(pd):
-                    view = flat.view(pd.shape)
-                else:   # e.g. channels_last conv weights: keep the physical layout cuDNN wants
-                    view = torch.as_strided(flat, pd.shape, pd.stride())
-                view.copy_(pd)
+            for s in L.slots:   # a custom placement's padding stays zero
+                view = s.view(self.param_arena[s.offset: s.offset + s.numel])
+                view.copy_(s.param.data)
                 s.param.data = view
         torch.cuda.synchronize(self.device)
         self.world.barrier()
@@ -182,9 +167,9 @@ class DeviceEngine:
         # ---- publication / reduction strategy ----
         mc = A.has_multicast
         if self.mode == "allgather" or self.size == 1:
-            self.bcast = 0                                  # BCAST_LOCAL
+            self.bcast = BCAST_LOCAL
         else:
-            self.bcast = 2 if (mc and os.environ.get("PSB200_BCAST", "auto") != "unicast") else 1
+            self.bcast = BCAST_MULTICAST if (mc and os.environ.get("PSB200_BCAST", "auto") != "unicast") else BCAST_UNICAST
         nvls_ok = mc and self.kind == KIND_DENSE and self.wire in (WIRE_F32, WIRE_BF16, WIRE_F16) and self.size > 1
         if reduce == "nvls" and not nvls_ok:
             raise ValueError("reduce='nvls' needs multicast memory and a dense fp32/bf16/fp16 wire")
@@ -201,16 +186,16 @@ class DeviceEngine:
         auto_nvls = (nvls_ok and self.mode == "ps" and self.size >= 4
                      and os.environ.get("PSB200_REDUCE", "") != "p2p")
         if reduce == "p2p":
-            self.reduce = 0
+            self.reduce = REDUCE_P2P
         else:
-            self.reduce = 1 if (reduce == "nvls" or (reduce == "auto" and (auto_nvls or (
-                nvls_ok and os.environ.get("PSB200_REDUCE", "") == "nvls")))) else 0
+            self.reduce = REDUCE_NVLS if (reduce == "nvls" or (reduce == "auto" and (auto_nvls or (
+                nvls_ok and os.environ.get("PSB200_REDUCE", "") == "nvls")))) else REDUCE_P2P
 
         # ---- the launch plan ----
         self.plan = None
         if self.is_server:
             P = self.m.UpdatePlan()
-            P.kind, P.wire, P.opt = self.kind, self.wire, (0 if opt.optim == "sgd" else 1)
+            P.kind, P.wire, P.opt = self.kind, self.wire, (OPT_SGD if opt.optim == "sgd" else OPT_ADAM)
             P.grid = min(nt, self.m.update_max_grid(self.kind, self.wire, P.opt))
             pub = self.off_stage if self.consistent else self.off_param      # where fresh parameters are published
             for r in range(self.size):
@@ -245,15 +230,13 @@ class DeviceEngine:
         self._sig_base = [p + self.off_signal for p in self.arena.ptrs]
         # ---- the pipeline chunks: contiguous runs of whole parameters in arena (= backward) order ----
         self._make_chunks()
-        self._fired: set = set()
-        self._keep: List[torch.Tensor] = []
+        self._start_step()
         self._keep_prev: List[torch.Tensor] = []   # last step's gradients: freed one step late (see _flush)
         self._prev_done = None                      # comm-stream completion of the last step
-        self._raw_bytes = 0
-        self._first_flush_done = False
         self.launches = 0                     # kernels of OURS launched (bench 'gpu_launches')
         self._closed = False
         self._gates: list = []
+        self._gate_epoch = -1                 # the last epoch whose PARAMS_READY a forward has acquired (gate / ensure_params)
         self._prof = CudaStepTimer(bool(getattr(opt, "profile", False)))
         self._epoch = 0                       # completed engine steps (the epoch-flag clock)
         # async bookkeeping
@@ -281,7 +264,6 @@ class DeviceEngine:
                 sl.param.ps_grad_out = functools.partial(self.grad_out, sl.param)
         self._snap_version = 0
         self._snap_shadow = None
-        self._step_hyp = None
         self._phyper_ptr = 0
         self._update_spans: list = []
         # device-timeout surfacing: an async copy of SIG_ERROR into pinned memory every few steps, read one poll late
@@ -329,8 +311,17 @@ class DeviceEngine:
         for k, c in enumerate(chunks):
             for sl in c:
                 self._chunk_of[sl.index] = k
-        self._chunk_items: List[list] = [[] for _ in chunks]
-        self._chunk_left = [len(c) for c in chunks]
+
+    def _start_step(self):
+        """The bookkeeping of a step no gradient has arrived for yet.  Callers decide what happens to the gradients kept
+        alive for the previous step (``_keep_prev``) and to its completion event (``_prev_done``)."""
+        self._fired: set = set()
+        self._keep: List[torch.Tensor] = []
+        self._raw_bytes = 0
+        self._first_flush_done = False
+        self._step_hyp = None
+        self._chunk_items: List[list] = [[] for _ in self.chunks]
+        self._chunk_left = [len(c) for c in self.chunks]
         self._next_chunk = 0
 
     def _progress(self, epoch: int, chunk: int) -> int:
@@ -338,15 +329,6 @@ class DeviceEngine:
         return (epoch - 1) * self.nchunks + chunk + 1
 
     # ---------------------------------------------------------------------------------- state
-    @staticmethod
-    def _like(flat: torch.Tensor, param: torch.Tensor) -> torch.Tensor:
-        """View a flat arena slice with the parameter's shape AND physical layout."""
-        if flat.numel() != param.numel():          # custom placement (layout.py): same strides over the same span
-            return torch.as_strided(flat, param.shape, param.stride())
-        if param.is_contiguous() or not _dense(param):
-            return flat.view(param.shape)
-        return torch.as_strided(flat, param.shape, param.stride())
-
     def _expose_state(self):
         """Make ``opt.state[p]`` views of the flat fp32 state (checkpoint parity, SURVEY §5)."""
         o = self.opt
@@ -355,15 +337,15 @@ class DeviceEngine:
             sl = slice(s.offset, s.offset + s.numel)
             if o.optim == "sgd":
                 if self.buf0 is not None:
-                    st["momentum_buffer"] = self._like(self.buf0[sl], s.param)
+                    st["momentum_buffer"] = s.view(self.buf0[sl])
             else:
                 st.setdefault("step", 0)
-                st["exp_avg"] = self._like(self.buf0[sl], s.param)
-                st["exp_avg_sq"] = self._like(self.buf1[sl], s.param)
+                st["exp_avg"] = s.view(self.buf0[sl])
+                st["exp_avg_sq"] = s.view(self.buf1[sl])
                 if self.buf2 is not None:
-                    st["max_exp_avg_sq"] = self._like(self.buf2[sl], s.param)
+                    st["max_exp_avg_sq"] = s.view(self.buf2[sl])
             if self.master is not None:
-                st["master_param"] = self._like(self.master[sl], s.param)
+                st["master_param"] = s.view(self.master[sl])
 
     def sync_state_to_torch(self):
         o = self.opt
@@ -399,7 +381,7 @@ class DeviceEngine:
                                  ("master_param", self.master)):
                     if buf is not None and key in st and st[key] is not None:
                         if st[key].data_ptr() != buf[sl].data_ptr():
-                            self._like(buf[sl], s.param).copy_(st[key].to(buf.dtype))
+                            s.view(buf[sl]).copy_(st[key].to(buf.dtype))
                 if "step" in st:
                     self._group_steps[s.group] = max(self._group_steps[s.group], int(st["step"]))
                     self._param_steps[s.index] = int(st["step"])
@@ -408,7 +390,7 @@ class DeviceEngine:
                 for s in self.layout.slots:
                     src = original.get(id(s.param), {}) if original is not None else o.state.get(s.param, {})
                     if "master_param" not in src:
-                        self._like(self.master[s.offset: s.offset + s.numel], s.param).copy_(s.param.data.float())
+                        s.view(self.master[s.offset: s.offset + s.numel]).copy_(s.param.data.float())
         if any(self._param_steps[s.index] != self._group_steps[s.group] for s in self.layout.slots):
             self._uniform_steps = False
         self._expose_state()
@@ -429,53 +411,47 @@ class DeviceEngine:
         if sl is None:
             return None
         flat = self.wire_arena[sl.first_tile * self.bpt: sl.first_tile * self.bpt + sl.numel * self.psz].view(self.dtype)
-        return self._like(flat, param) if sl.strides is None else torch.as_strided(flat, param.shape, sl.strides)
+        return sl.view(flat)
 
     def on_grad(self, grad: torch.Tensor, name: str, param: torch.nn.Parameter):
         """Backward hook (``ps.py:98-101``): file the gradient under its chunk; every chunk that is now complete (in
         arena order) is encoded — and on the server gathered / updated / broadcast — right away, under backward."""
         s = self.layout.by_id[id(param)]
         g = grad.detach()
-        if self._direct_ok and g.data_ptr() == self._wire_ptr + s.first_tile * self.bpt and g.dtype == self.dtype \
-                and g.stride() == param.stride():
-            # the producer already wrote this gradient into the wire arena (grad_out): nothing to encode
-            if s.index in self._fired:
-                raise RuntimeError(f"parameter {name!r} produced two gradients before step()")
-            self._fired.add(s.index)
-            k = self._chunk_of[s.index]
-            self._chunk_left[k] -= 1
-            self._raw_bytes += s.numel * self.psz
+        # a gradient the producer already wrote into the wire arena (grad_out) has nothing to encode
+        direct = self._direct_ok and g.data_ptr() == self._wire_ptr + s.first_tile * self.bpt and g.dtype == self.dtype \
+            and g.stride() == param.stride()
+        if not direct:
+            if g.dtype != self.dtype:
+                g = g.to(self.dtype)
+            if s.strides is not None:
+                # custom placement: the encode kernel reads the whole span, padding included (it must be zero)
+                if not (g.stride() == param.stride() and g.data_ptr() % 16 == 0 and g.storage_offset() * g.element_size() +
+                        s.numel * g.element_size() <= g.untyped_storage().nbytes()):
+                    span = torch.zeros(s.numel, dtype=g.dtype, device=g.device)
+                    s.view(span).copy_(g)
+                    g = span
+                else:
+                    g = torch.as_strided(g, (s.numel,), (1,))
+            elif g.stride() != param.stride() or g.data_ptr() % 16:
+                # the arena is in the parameter's physical order: bring the gradient into it
+                g = torch.empty_strided(param.shape, param.stride(), dtype=g.dtype, device=g.device).copy_(g)
+        if s.index in self._fired:           # gradient accumulation: later micro-batches add up
+            raise RuntimeError(f"parameter {name!r} produced two gradients before step(); "
+                               "call step() after every backward (the reference encodes per backward)")
+        self._fired.add(s.index)
+        k = self._chunk_of[s.index]
+        self._chunk_left[k] -= 1
+        self._raw_bytes += s.numel * self.psz
+        if direct:
             self.direct_grads += 1
             self.direct_names.add(name)
             if param.grad is not None:
                 # AccumulateGrad would add the incoming gradient INTO param.grad in place — and both may alias the same wire
                 # tile (zero_grad(set_to_none=False)): drop the old one so the new gradient is assigned, not accumulated
                 param.grad = None
-            while self._next_chunk < self.nchunks and self._chunk_left[self._next_chunk] == 0:
-                self._flush_chunk(self._next_chunk)
-            return
-        if g.dtype != self.dtype:
-            g = g.to(self.dtype)
-        if s.strides is not None:
-            # custom placement: the encode kernel reads the whole span, padding included (it must be zero)
-            if not (g.stride() == param.stride() and g.data_ptr() % 16 == 0 and g.storage_offset() * g.element_size() +
-                    s.numel * g.element_size() <= g.untyped_storage().nbytes()):
-                span = torch.zeros(s.numel, dtype=g.dtype, device=g.device)
-                torch.as_strided(span, param.shape, s.strides).copy_(g)
-                g = span
-            else:
-                g = torch.as_strided(g, (s.numel,), (1,))
-        elif g.stride() != param.stride() or g.data_ptr() % 16:
-            # the arena is in the parameter's physical order: bring the gradient into it
-            g = torch.empty_strided(param.shape, param.stride(), dtype=g.dtype, device=g.device).copy_(g)
-        if s.index in self._fired:           # gradient accumulation: later micro-batches add up
-            raise RuntimeError(f"parameter {name!r} produced two gradients before step(); "
-                               "call step() after every backward (the reference encodes per backward)")
-        self._fired.add(s.index)
-        k = self._chunk_of[s.index]
-        self._chunk_items[k].append((s, g))
-        self._chunk_left[k] -= 1
-        self._raw_bytes += s.numel * self.psz
+        else:
+            self._chunk_items[k].append((s, g))
         while self._next_chunk < self.nchunks and self._chunk_left[self._next_chunk] == 0:
             self._flush_chunk(self._next_chunk)
 
@@ -549,8 +525,12 @@ class DeviceEngine:
                 m.wait_flags(self.arena.local_ptr + self.off_signal, m.SIG_GRAD_READY, wait_mask, self._progress(epoch, k),
                              self.timeout_s, csh)
                 self.launches += 1
-            self.plan.launch(epoch, self._get_hypers(), (1 << n) - 1, inv, 0,
-                             (0 if n == 1 else (1 if self.mode == "ps" else 2)) if last else 0,
+            if not last or n == 1:
+                signal_mode = SIGNAL_NONE
+            else:
+                signal_mode = SIGNAL_PARAMS_READY if self.mode == "ps" else SIGNAL_CONSUMED
+            # (epoch, groups, contrib_mask, inv_count, wait_grads, signal_mode, ...)
+            self.plan.launch(epoch, self._get_hypers(), (1 << n) - 1, inv, 0, signal_mode,
                              active_ptr=active_ptr, timeout_s=self.timeout_s,
                              wait_mask=wait_mask, stream=csh,
                              tile_begin=lo, tile_end=hi, wait_value=self._progress(epoch, k),
@@ -609,17 +589,15 @@ class DeviceEngine:
     def _hypers(self) -> List[List[float]]:
         o = self.opt
         out = []
+        for gi in range(len(o.param_groups)):
+            self._group_steps[gi] += 1
+        first = any(t == 1 for t in self._group_steps)
         if o.optim == "sgd":
             # SGD's tuple only changes with lr schedules / the first step: reuse the cached list otherwise
             key = tuple((g["lr"], g["weight_decay"], g["momentum"], g["dampening"], g["nesterov"]) for g in o.param_groups)
-            for gi in range(len(o.param_groups)):
-                self._group_steps[gi] += 1
-            first = any(t == 1 for t in self._group_steps)
             if not first and self._hyper_cache is not None and self._hyper_cache[0] == key:
                 return self._hyper_cache[1]
         for gi, g in enumerate(o.param_groups):
-            if o.optim != "sgd":
-                self._group_steps[gi] += 1
             t = self._group_steps[gi]
             if o.optim == "sgd":
                 out.append([float(g["lr"]), float(g["weight_decay"]), float(g["momentum"]), float(g["dampening"]),
@@ -629,7 +607,7 @@ class DeviceEngine:
                 step_size = float(g["lr"]) * math.sqrt(1 - b2 ** t) / (1 - b1 ** t)     # ps.py:257-259
                 out.append([float(g["lr"]), float(g["weight_decay"]), 0.0, 0.0, float(b1), float(b2),
                             float(g["eps"]), step_size, 0.0, float(bool(g.get("amsgrad", False))), float(t == 1)])
-        if o.optim == "sgd" and not any(t == 1 for t in self._group_steps):
+        if o.optim == "sgd" and not first:
             self._hyper_cache = (key, out)
         return out
 
@@ -693,7 +671,6 @@ class DeviceEngine:
         self._flush_rest(cs, joined=True)
         self._get_hypers()                   # workers too: keeps the per-group step counters aligned with the server
         data["optim_step_time"] = time.time() - t2
-        data["isend_time"] = 0.0
         done = self._event()
         done.record(cs)
         t3 = time.time()
@@ -731,19 +708,12 @@ class DeviceEngine:
             self._uniform_steps = False              # some parameter sat this step out: per-parameter counts diverge from now on
         for i in self._fired:
             self._param_steps[i] += 1
-        self._fired = set()
-        self._keep_prev, self._keep = self._keep, []
+        self._keep_prev = self._keep
         if done is None:                     # comm-stream completion marker of this step (see _flush)
             done = self._event()
             done.record(self.comm_stream)
         self._prev_done = done
-        self._raw_bytes = 0
-        self._first_flush_done = False
-        self._step_hyp = None
-        self._next_chunk = 0
-        self._chunk_left = [len(c) for c in self.chunks]
-        for it in self._chunk_items:
-            it.clear()
+        self._start_step()
         if os.environ.get("PSB200_CHECK") == "1":
             self.check()
         elif self.size > 1 and self._epoch % self._err_every == 0:
@@ -784,16 +754,9 @@ class DeviceEngine:
         self._err_host.zero_()
         self._err_event = None
         self._epoch = 0
-        self._fired = set()
-        self._keep, self._keep_prev = [], []
+        self._start_step()
+        self._keep_prev = []
         self._prev_done = None
-        self._raw_bytes = 0
-        self._first_flush_done = False
-        self._step_hyp = None
-        self._next_chunk = 0
-        self._chunk_left = [len(c) for c in self.chunks]
-        for it in self._chunk_items:
-            it.clear()
         self._gate_epoch = -1
         self.version = 0
         self._async_pending, self._async_done_workers = [], set()
@@ -838,12 +801,12 @@ class DeviceEngine:
     # ------------------------------------------------------------------------------ async mode
     def _step_async(self, data):
         o = self.opt
-        sig_base = [p + self.off_signal for p in self.arena.ptrs]
+        sig_base = self._sig_base
         cs = self.comm_stream
         cur = torch.cuda.current_stream(self.device)
         if self.rank != 0:
             epoch = self._epoch + 1
-            ev = torch.cuda.Event()
+            ev = self._event()
             ev.record(cur)
             cs.wait_event(ev)
             self._flush_rest(cs, joined=True)        # chunks not yet encoded during backward (+ inactive parameters)
@@ -862,12 +825,7 @@ class DeviceEngine:
         # ---- rank 0: the server — device-resident: select → (open sequence lock) → update → ack are all queued without
         # looking at their result; results come back through a ring of pinned slots, read when their event has completed.
         # The host only blocks when it is `_async_depth` iterations AHEAD of the GPU (never the other way round). ----
-        self._fired = set()
-        self._keep = []
-        self._next_chunk = 0
-        self._chunk_left = [len(c) for c in self.chunks]
-        for it in self._chunk_items:
-            it.clear()
+        self._start_step()
         n = self.size
         self._async_harvest(block=False)
         cand = ((1 << n) - 1) & ~1
@@ -887,8 +845,10 @@ class DeviceEngine:
         hyp = self._hypers()
         self.m.select_ready(sig_base[0], self._consumed.data_ptr(), cand, quota, self._select_out.data_ptr(),
                             self.timeout_s, self.version, sig_base if self.consistent else [], self._cs)
-        self.plan.launch(o.steps, hyp, 0, 1.0, 0, 1, 0, self.version, self._select_out.data_ptr(),
-                         1 if o.average else 0, 0, self.timeout_s, stream=self._cs)
+        # the contributors and their count come from the select kernel (select_out), not from contrib_mask / inv_count
+        self.plan.launch(o.steps, hyp, 0, 1.0, 0, SIGNAL_PARAMS_READY,
+                         ack_mask=0, version=self.version, select_out=self._select_out.data_ptr(),
+                         average_dynamic=1 if o.average else 0, active_ptr=0, timeout_s=self.timeout_s, stream=self._cs)
         self.launches += 2
         with torch.cuda.stream(cs):
             slot["host"].copy_(self._select_out, non_blocking=True)
@@ -986,7 +946,7 @@ class DeviceEngine:
         the plain wait kernel on the current stream unless this epoch's broadcast was already acquired."""
         if self.size == 1 or self.mode != "ps" or self.rank == 0 or self._epoch == 0 or not self._gates:
             return
-        if getattr(self, "_gate_epoch", -1) == self._epoch:
+        if self._gate_epoch == self._epoch:
             return
         self._gate_epoch = self._epoch
         self.m.wait_flags(self._sig_base[self.rank], self.m.SIG_PARAMS_READY, 1, self._epoch, self.timeout_s)

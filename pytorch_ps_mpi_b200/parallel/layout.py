@@ -37,6 +37,30 @@ class ParamSlot:
     def offset(self) -> int:      # element offset in the arena
         return self.first_tile * TILE
 
+    def view(self, flat: torch.Tensor) -> torch.Tensor:
+        """The parameter-shaped view of ``flat``, this slot's ``numel`` elements of an arena (parameters, gradients or optimizer
+        state), in the parameter's physical layout: the custom placement if the module asked for one, else the parameter's own
+        strides when they are a dense permutation (e.g. channels_last conv weights, as cuDNN wants them), else contiguous."""
+        p = self.param
+        if self.strides is not None:
+            return torch.as_strided(flat, p.shape, self.strides)
+        if p.is_contiguous() or not _dense(p):
+            return flat.view(p.shape)
+        return torch.as_strided(flat, p.shape, p.stride())
+
+
+def _dense(t: torch.Tensor) -> bool:
+    """True if ``t``'s strides describe a dense, non-overlapping permutation of its shape."""
+    if t.is_contiguous():
+        return True
+    dims = sorted(((st, sz) for st, sz in zip(t.stride(), t.shape) if sz > 1), key=lambda x: x[0])
+    expect = 1
+    for st, sz in dims:
+        if st != expect:
+            return False
+        expect *= sz
+    return True
+
 
 class FlatLayout:
     def __init__(self, param_groups, names: Dict[int, str]):

@@ -99,6 +99,14 @@ def test_every_native_call_site_binds(native):
     assert checked >= 30, checked          # the scan really saw the engine's call sites
 
 
+def test_launch_mode_names_match_the_extension(native):
+    """The engine's launch-mode constants mirror the enums of ``common.cuh`` that the extension exports."""
+    from pytorch_ps_mpi_b200.parallel import device_engine as de
+    names = [n for n in dir(de) if n.split("_")[0] in ("OPT", "BCAST", "REDUCE", "SIGNAL")]
+    assert len(names) == 10
+    assert {n: getattr(native, n) for n in names} == {n: getattr(de, n) for n in names}
+
+
 def test_signature_parser():
     s = _signature("f(self: X, a: typing.SupportsInt | typing.SupportsIndex, b: collections.abc.Sequence[int] = [], "
                    "c: typing.SupportsFloat = 30.0) -> None\n")

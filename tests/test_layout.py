@@ -86,3 +86,32 @@ def test_custom_arena_placement_hint():
     p.ps_arena_layout = ((8, 1), 16)                      # reaches element 3*8 + 3 = 27 >= 16
     with pytest.raises(ValueError):
         FlatLayout([{"params": [p]}], {id(p): "p"})
+
+
+def test_slot_view_keeps_the_physical_layout():
+    """``ParamSlot.view``: a flat arena slice seen with the parameter's shape — contiguous, the parameter's own dense strides
+    (channels_last), or the module's custom placement over a padded span (the stem's [64,176] GEMM matrix)."""
+    from pytorch_ps_mpi_b200.ops.stem import STEM_K, STEM_STRIDES
+    contiguous = torch.nn.Parameter(torch.randn(5, 7))
+    cl = torch.nn.Parameter(torch.randn(8, 4, 3, 3).contiguous(memory_format=torch.channels_last))
+    stem = torch.nn.Parameter(torch.randn(64, 3, 7, 7))
+    stem.ps_arena_layout = (STEM_STRIDES, 64 * STEM_K)
+    strided = torch.nn.Parameter(torch.randn(6, 10)[:, ::2])         # not dense: the arena holds it contiguously
+    params = [contiguous, cl, stem, strided]
+    L = FlatLayout([{"params": params}], {id(p): f"p{i}" for i, p in enumerate(params)})
+    arena = torch.zeros(L.numel_padded)
+    want = {id(contiguous): (5 * 7, (7, 1)), id(cl): (8 * 4 * 3 * 3, cl.stride()), id(stem): (64 * STEM_K, STEM_STRIDES),
+            id(strided): (6 * 5, (5, 1))}
+    for s in L.slots:
+        flat = arena[s.offset: s.offset + s.numel]
+        v = s.view(flat)
+        assert s.numel == want[id(s.param)][0] and v.shape == s.param.shape and v.stride() == tuple(want[id(s.param)][1])
+        assert v.data_ptr() == flat.data_ptr()
+        v.copy_(s.param.detach())
+        assert torch.equal(v, s.param.detach())
+    s = L.by_id[id(stem)]
+    stem_span = arena[s.offset: s.offset + s.numel].view(64, STEM_K)
+    assert torch.equal(stem_span[:, :168].reshape(64, 7, 8, 3)[:, :, :7].permute(0, 3, 1, 2), stem.detach())   # (kh, kw, c)
+    assert not stem_span[:, 168:].any() and not stem_span[:, :168].reshape(64, 7, 8, 3)[:, :, 7:].any()      # padding stays 0
+    s = L.by_id[id(cl)]
+    assert torch.equal(arena[s.offset: s.offset + s.numel], cl.detach().permute(0, 2, 3, 1).reshape(-1))   # NHWC in the arena
