@@ -8,7 +8,10 @@ Sections (``--only a,b,...``; default all):
 * ``wgrad``           weight gradient of the fused autograd path (im2col rebuilt in backward) vs the default path;
 * ``wgrad_implicit``  ``psb_stem_wgrad_kernel`` (MN-major wgmma operands) vs a fp32 reference, + timing at batch 256;
 * ``model``           one ResNet-18 forward/backward with the fused stem vs the default path;
-* ``timing``          batch 256, 224x224: stem + BN1 forward, default vs fused (CUDA events, L2 flushed).
+* ``timing``          batch 256, 224x224: stem + BN1 forward, default vs fused (CUDA events, L2 flushed);
+* ``tail``            ResNet-18's stem tail (BN1 + ReLU + max-pool on 256x64x112x112): the unfused chain against the fused
+                      kernels, forward and backward — bit-identical results, the least HBM bytes each moves (from the shapes),
+                      time (CUDA events, L2 flushed) and achieved bandwidth as a share of the data sheet's 3.35 TB/s.
 
 Exit code 1 if any check fails.  One JSON line per check on stdout, appended to ``bench_out/stem_fused_check.jsonl``.
 A device-side trap kills the CUDA context, so on first contact run one section per process, each under ``timeout``:
@@ -145,8 +148,46 @@ def sec_timing():
          default_conv_only_ms=t_conv_only, ok=True)
 
 
+def sec_tail():
+    m = ext.cuda()
+    N, C, H, W = 256, 64, 112, 112
+    T = N * C * H * W * 2                     # the stem output (bf16)
+    P, A, M = T // 4, T // 8, T // 16         # pooled output, 1-byte taps, 1-bit ReLU mask
+    torch.manual_seed(0)
+    x = cl(torch.randn(N, C, H, W, device=DEV).bfloat16())
+    xf = x.float()
+    sums = torch.cat([xf.sum((0, 2, 3)), (xf * xf).sum((0, 2, 3))])
+    del xf
+    g = (torch.randn(C, device=DEV) * 0.5 + 1.0).bfloat16()
+    b = (torch.randn(C, device=DEV) * 0.5).bfloat16()
+    dp = cl(torch.randn(N, C, H // 2, W // 2, device=DEV).bfloat16())
+    rm, rv = torch.zeros(C, device=DEV), torch.ones(C, device=DEV)
+
+    def fwd_unfused():
+        y, mean, rstd, mask = m.bn_forward_presummed(x, None, g, b, rm, rv, 1e-5, 0.1, True, sums)
+        return (*m.maxpool_forward(y), mean, rstd, mask)
+
+    def fwd_fused():
+        return m.bn_forward_presummed(x, None, g, b, rm, rv, 1e-5, 0.1, True, sums, pool=True)
+
+    pu, au, mean, rstd, mask = fwd_unfused()
+    pf, _, _, af = fwd_fused()
+    bwd_unfused = lambda: m.bn_backward(m.maxpool_backward(dp, au, H, W), x, mask, g, mean, rstd, True, False)   # noqa: E731
+    bwd_fused = lambda: m.bn_backward(dp, x, x, g, mean, rstd, True, False, pool_arg=af)                        # noqa: E731
+    du, df = bwd_unfused(), bwd_fused()
+    same = (torch.equal(pu.view(torch.int16), pf.view(torch.int16))
+            and all(torch.equal(u.view(torch.int16), f.view(torch.int16)) for u, f in zip((du[0], du[2], du[3]), (df[0], df[2], df[3]))))
+    rows = {"fwd_unfused": (fwd_unfused, 2 * T + M + T + P + A), "fwd_fused": (fwd_fused, T + P + A),
+            "bwd_unfused": (bwd_unfused, P + A + T + 2 * T + M + 3 * T + M), "bwd_fused": (bwd_fused, T + P + A + 2 * T + P + A)}
+    out = {}
+    for name, (fn, nbytes) in rows.items():
+        ms = bench(fn, iters=20)
+        out[name] = {"ms": ms, "min_bytes_MB": nbytes / 1e6, "GB_per_s": nbytes / ms / 1e6, "share_of_3.35TBps": nbytes / ms / 3.35e9}
+    emit(check="tail", shape=[N, C, H, W], bit_identical=bool(same), **out, ok=bool(same))
+
+
 SECTIONS = {"numerics": sec_numerics, "wgrad": sec_wgrad, "wgrad_implicit": sec_wgrad_implicit, "model": sec_model,
-            "timing": sec_timing}
+            "timing": sec_timing, "tail": sec_tail}
 
 
 def main():

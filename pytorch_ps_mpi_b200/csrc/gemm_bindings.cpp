@@ -141,14 +141,27 @@ std::vector<at::Tensor> bn_forward(const at::Tensor& x, c10::optional<at::Tensor
 // wire arena (DeviceEngine.grad_out) so these gradients need no encode pass.
 std::vector<at::Tensor> bn_backward(const at::Tensor& dy, const at::Tensor& x, const at::Tensor& y, const at::Tensor& gamma,
                                     const at::Tensor& mean, const at::Tensor& rstd, bool relu, bool has_res,
-                                    c10::optional<at::Tensor> out_dgamma, c10::optional<at::Tensor> out_dbeta) {
+                                    c10::optional<at::Tensor> out_dgamma, c10::optional<at::Tensor> out_dbeta,
+                                    c10::optional<at::Tensor> pool_arg) {
   // relu: `y` is either the saved output (bf16, same shape as x) or the forward's 1-bit mask (uint8, numel/8 bytes)
-  const bool masked = relu && y.scalar_type() == at::kByte;
+  // pool_arg: the taps of bn_forward_presummed(pool=True); `dy` is then the pooled gradient and `y` is unused
+  const bool pooled = pool_arg.has_value() && pool_arg->defined();
+  const bool masked = !pooled && relu && y.scalar_type() == at::kByte;
   if (masked) TORCH_CHECK(y.numel() * 8 == x.numel() && y.is_contiguous(), "bn_backward: mask size mismatch");
   check_nhwc(dy, "dy");
   check_nhwc(x, "x");
   const int C = (int)x.size(1);
   const long long pixels = x.numel() / C;
+  const int N = (int)x.size(0), H = (int)x.size(2), W = (int)x.size(3);
+  if (pooled) {
+    TORCH_CHECK(relu && !has_res, "bn_backward(pool_arg): ReLU and no residual only");
+    TORCH_CHECK(H % 2 == 0 && W % 2 == 0 && C % 8 == 0 && C <= 2048 && pixels < (1LL << 31),
+                "bn_backward(pool_arg): H and W must be even, C a multiple of 8 and <= 2048");
+    TORCH_CHECK(dy.size(0) == N && dy.size(1) == C && dy.size(2) == H / 2 && dy.size(3) == W / 2, "bn_backward: pooled dy shape");
+    TORCH_CHECK(pool_arg->scalar_type() == at::kByte && pool_arg->sizes() == dy.sizes() &&
+                    pool_arg->is_contiguous(at::MemoryFormat::ChannelsLast),
+                "bn_backward: pool_arg must be the forward's channels-last uint8 taps");
+  }
   auto dx = at::empty_like(x);
   at::Tensor dres;
   if (has_res) dres = at::empty_like(x);
@@ -164,6 +177,14 @@ std::vector<at::Tensor> bn_backward(const at::Tensor& dy, const at::Tensor& x, c
   auto scratch = at::empty({3 * C}, x.options().dtype(at::kFloat));
   auto part = at::empty({psb_bn_partial_floats(pixels, C)}, x.options().dtype(at::kFloat));
   float* sp = scratch.data_ptr<float>();
+  if (pooled) {
+    psb_bn_relu_maxpool_backward(c10::cuda::getCurrentCUDAStream().stream(), dy.data_ptr(), pool_arg->data_ptr(), x.data_ptr(),
+                                 gamma.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), part.data_ptr<float>(), sp,
+                                 dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), N, H, W, C);
+    cudaError_t e = cudaGetLastError();
+    TORCH_CHECK(e == cudaSuccess, "psb_bn_relu_maxpool_backward: ", cudaGetErrorString(e));
+    return {dx, dres, dgamma, dbeta};
+  }
   psb_bn_backward(c10::cuda::getCurrentCUDAStream().stream(), dy.data_ptr(), x.data_ptr(),
                   (relu && !masked) ? y.data_ptr() : nullptr, gamma.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
                   part.data_ptr<float>(), sp, dx.data_ptr(), has_res ? dres.data_ptr() : nullptr, dgamma.data_ptr(), dbeta.data_ptr(), pixels, C,
@@ -214,16 +235,36 @@ at::Tensor normalize_pad8(const at::Tensor& x, std::vector<double> mean, std::ve
 }
 
 // bf16 NHWC [N,3,H,W] (channels_last) → patch matrix [N*OH*OW, 176] for the 7x7/s2/p3 stem
-// training BatchNorm forward whose Σx / Σx² were produced by the fused stem kernel; returns (y, mean, rstd)
+// training BatchNorm forward whose Σx / Σx² were produced by the fused stem kernel; returns (y, mean, rstd, mask)
+// pool: the ResNet stem tail — BN + ReLU + 3x3/s2/p1 max-pool in one pass (no residual, even H and W); returns
+// (pooled, mean, rstd, arg) where arg holds each window's tap, 255 where the window routes no gradient (bn_backward's pool_arg)
 std::vector<at::Tensor> bn_forward_presummed(const at::Tensor& x, c10::optional<at::Tensor> res, const at::Tensor& gamma,
                                              const at::Tensor& beta, at::Tensor running_mean, at::Tensor running_var, double eps,
-                                             double momentum, bool relu, const at::Tensor& sums) {
+                                             double momentum, bool relu, const at::Tensor& sums, bool pool) {
   check_nhwc(x, "x");
   const int C = (int)x.size(1);
   TORCH_CHECK(C % 8 == 0 && C <= 2048, "channels must be a multiple of 8 and <= 2048");
   TORCH_CHECK(sums.is_cuda() && sums.scalar_type() == at::kFloat && sums.numel() == 2 * C && sums.is_contiguous(),
               "sums must be a contiguous fp32 CUDA tensor of 2*C elements");
   const long long pixels = x.numel() / C;
+  if (pool) {
+    const int N = (int)x.size(0), H = (int)x.size(2), W = (int)x.size(3);
+    TORCH_CHECK(relu && !(res.has_value() && res->defined()), "bn_forward_presummed(pool=True): ReLU and no residual only");
+    TORCH_CHECK(H % 2 == 0 && W % 2 == 0 && H > 0 && W > 0, "bn_forward_presummed(pool=True): H and W must be even");
+    TORCH_CHECK(pixels < (1LL << 31), "bn_forward_presummed(pool=True): more than 2^31 pixels");
+    TORCH_CHECK(running_mean.scalar_type() == at::kFloat && running_var.scalar_type() == at::kFloat, "running stats must be fp32");
+    auto y = at::empty({N, C, H / 2, W / 2}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
+    auto arg = at::empty({N, C, H / 2, W / 2}, x.options().dtype(at::kByte).memory_format(at::MemoryFormat::ChannelsLast));
+    auto scratch = at::empty({4 * C}, x.options().dtype(at::kFloat));   // mean | rstd | scale | shift
+    float* sp = scratch.data_ptr<float>();
+    psb_bn_relu_maxpool_forward_presummed(c10::cuda::getCurrentCUDAStream().stream(), x.data_ptr(), gamma.data_ptr(),
+                                          beta.data_ptr(), sums.data_ptr<float>(), sp, sp + C, sp + 2 * C, sp + 3 * C,
+                                          running_mean.data_ptr<float>(), running_var.data_ptr<float>(), N, H, W, C, (float)eps,
+                                          (float)momentum, y.data_ptr(), arg.data_ptr());
+    cudaError_t e = cudaGetLastError();
+    TORCH_CHECK(e == cudaSuccess, "psb_bn_relu_maxpool_forward_presummed: ", cudaGetErrorString(e));
+    return {y, scratch.narrow(0, 0, C), scratch.narrow(0, C, C), arg};
+  }
   const void* rp = nullptr;
   if (res.has_value() && res->defined()) {
     check_nhwc(*res, "residual");
@@ -349,7 +390,10 @@ void bind_gemm(py::module_& m) {
   m.def("maxpool_forward", &maxpool_forward, "channels-last bf16 3x3/s2/p1 max pool → (y, argpos)");
   m.def("maxpool_backward", &maxpool_backward, "gather-style backward of maxpool_forward");
   m.def("bn_forward", &bn_forward, "fused channels-last bf16 BatchNorm(+residual)(+ReLU) forward");
-  m.def("bn_forward_presummed", &bn_forward_presummed, "BN forward with sums produced by the fused stem kernel");
+  m.def("bn_forward_presummed", &bn_forward_presummed, py::arg("x"), py::arg("res"), py::arg("gamma"), py::arg("beta"),
+        py::arg("running_mean"), py::arg("running_var"), py::arg("eps"), py::arg("momentum"), py::arg("relu"), py::arg("sums"),
+        py::arg("pool") = false,
+        "BN forward with sums produced by the fused stem kernel; pool=True: + ReLU + 3x3/s2/p1 max-pool → (pooled, mean, rstd, arg)");
   m.def("stem_fwd", &stem_fwd, py::arg("x"), py::arg("w2d"), py::arg("want_sums") = true, py::arg("flag_ptr") = 0,
         py::arg("epoch") = 0, py::arg("timeout_s") = 30.0,
         "fused implicit-GEMM ResNet stem (+ BN statistics) on wgmma; flag_ptr/epoch: PARAMS_READY gate of the weight load");
@@ -358,7 +402,8 @@ void bind_gemm(py::module_& m) {
   m.def("stem_wgrad", &stem_wgrad, "implicit weight gradient of the stem → per-CTA fp32 partials [grid,176,64]");
   m.def("bn_backward", &bn_backward, py::arg("dy"), py::arg("x"), py::arg("y"), py::arg("gamma"), py::arg("mean"), py::arg("rstd"),
         py::arg("relu"), py::arg("has_res"), py::arg("out_dgamma") = c10::nullopt, py::arg("out_dbeta") = c10::nullopt,
-        "fused channels-last bf16 BatchNorm(+residual)(+ReLU) backward");
+        py::arg("pool_arg") = c10::nullopt,
+        "fused channels-last bf16 BatchNorm(+residual)(+ReLU) backward; pool_arg: dy is the pooled gradient of the stem tail");
   m.def("bcast_gemm", &bcast_gemm, py::arg("x"), py::arg("w_ptr"), py::arg("N"), py::arg("K"), py::arg("bias"),
         py::arg("relu"), py::arg("flag_ptr") = 0, py::arg("epoch") = 0, py::arg("timeout_s") = 30.0, py::arg("variant") = 0,
         "wgmma/TMA GEMM whose weight tiles are gated on the PS broadcast epoch flag");

@@ -321,9 +321,179 @@ __global__ void __launch_bounds__(BN_THREADS) psb_bn_bwd_apply(const __nv_bfloat
   }
 }
 
-// (A fused BatchNorm-apply + ReLU + 3x3/s2 max-pool pair lived here in round 2: per-pixel gather, then a 2x2-quad backward.
-//  It was correct but never beat the unfused kernels once those got the 1-bit ReLU mask and the quad max-pool backward,
-//  and was deleted.)
+// ---- ResNet stem tail: BatchNorm + ReLU + 3x3/s2/p1 max-pool (training, H and W even) -------------------------------------
+// The unfused chain writes the full-resolution BN output y only for the pool to read it, and the pool backward writes the
+// full-resolution gradient only for the BN backward to read it.  Here the forward pools straight from x, and both backward
+// passes gather the pooled gradient themselves, so neither tensor exists.  (Round 2 had a fused forward that gathered per output
+// pixel and was deleted because it lost to the unfused kernels; what is different now: the backward, which moves most of the
+// bytes, is fused too, and the forward walks rows like psb_maxpool_fwd_rows.)  Every value is bit-identical to the unfused chain:
+// the taps are rounded to bf16 exactly as psb_bn_apply stores them, the pool's rule picks the maximum, and the gather forms
+// each pixel's gradient with psb_maxpool_bwd_quads' expression.  A window whose maximum is not > 0 stores tap 255 ("routes
+// nothing") in place of the ReLU mask: in the unfused chain its gradient lands on a pixel whose mask bit is 0.
+struct TailGeom {
+  int N, H, W, OH, OW;   // input (even H, W) and pooled extents
+};
+
+__global__ void __launch_bounds__(BN_THREADS, 1) psb_bn_relu_maxpool_fwd(const __nv_bfloat16* __restrict__ x,
+                                                                          const float* __restrict__ scale,
+                                                                          const float* __restrict__ shift,
+                                                                          __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ arg,
+                                                                          BnGeom g, TailGeom t) {
+  const int tx = threadIdx.x % g.groups, ty = threadIdx.x / g.groups;
+  if (ty >= g.lanes) return;
+  float sc[8], sh[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    sc[j] = scale[tx * 8 + j];
+    sh[j] = shift[tx * 8 + j];
+  }
+  const int rows = t.N * t.OH;
+  for (int row = blockIdx.x; row < rows; row += gridDim.x) {   // one pooled row per CTA: L1 / L2 absorb the window overlap
+    const int n = row / t.OH, oh = row - n * t.OH;
+    const int h0 = oh * 2 - 1;
+    const __nv_bfloat16* xin = x + (size_t)n * t.H * t.W * g.C + tx * 8;
+    for (int ow = ty; ow < t.OW; ow += g.lanes) {
+      const int w0 = ow * 2 - 1;
+      float best[8];
+      uint32_t pos[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) best[j] = -INFINITY, pos[j] = 255;
+#pragma unroll
+      for (int kh = 0; kh < 3; ++kh) {
+        const int h = h0 + kh;
+        if (h < 0 || h >= t.H) continue;
+#pragma unroll
+        for (int kw = 0; kw < 3; ++kw) {
+          const int w = w0 + kw;
+          if (w < 0 || w >= t.W) continue;
+          float v[8];
+          ld8(xin + ((size_t)h * t.W + w) * g.C, v);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[j] = fmaxf(fmaf(v[j], sc[j], sh[j]), 0.f);   // psb_bn_apply<false, true>
+          unpack_bf16x8(make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
+                                   pack_bf16x2(v[6], v[7])), v);                          // the bf16 value y would hold
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (v[j] > best[j]) {          // strictly greater: the first maximum wins ties (psb_maxpool_fwd_rows)
+              best[j] = v[j];
+              pos[j] = kh * 3 + kw;
+            }
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (!(best[j] > 0.f)) pos[j] = 255;
+      const size_t o = ((size_t)row * t.OW + ow) * g.C + tx * 8;
+      st8(y + o, best);
+      *reinterpret_cast<uint2*>(arg + o) = make_uint2(pos[0] | (pos[1] << 8) | (pos[2] << 16) | (pos[3] << 24),
+                                                      pos[4] | (pos[5] << 8) | (pos[6] << 16) | (pos[7] << 24));
+    }
+  }
+}
+
+// The masked BN-input gradient dy' of 8 channels at input pixel p, gathered from the pooled gradient `dp` and the forward's taps:
+// what psb_maxpool_bwd_quads writes for this pixel's position in its 2x2 quad, same terms in the same order, rounded to bf16.
+// Window (a, b) of the quad's four (oh0 + a, ow0 + b) covers the pixel at (ph, pw) iff a <= ph and b <= pw, with tap
+// (ph + 1 - 2a) * 3 + (pw + 1 - 2b).
+__device__ __forceinline__ void pooled_grad8(const __nv_bfloat16* __restrict__ dp, const uint8_t* __restrict__ arg, int p, int C,
+                                             int tx, const TailGeom& t, float* d) {
+  const int w = p % t.W, nh = p / t.W, h = nh % t.H, n = nh / t.H;
+  const int ph = h & 1, pw = w & 1, oh0 = h >> 1, ow0 = w >> 1;
+  uint2 pr[4];
+  float f[4][8];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int a = i >> 1, b = i & 1;
+    pr[i] = make_uint2(0xffffffffu, 0xffffffffu);          // tap 255 matches nothing
+    uint4 dv = make_uint4(0u, 0u, 0u, 0u);
+    if (a <= ph && b <= pw && oh0 + a < t.OH && ow0 + b < t.OW) {
+      const size_t o = (((size_t)n * t.OH + oh0 + a) * t.OW + ow0 + b) * C + tx * 8;
+      pr[i] = *reinterpret_cast<const uint2*>(arg + o);
+      dv = *reinterpret_cast<const uint4*>(dp + o);
+    }
+    unpack_bf16x8(dv, f[i]);
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    float acc = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int a = i >> 1, b = i & 1;
+      if (a > ph || b > pw) continue;
+      const uint32_t tap = ((j < 4 ? pr[i].x : pr[i].y) >> (8 * (j & 3))) & 0xffu;
+      const float v = tap == (uint32_t)((ph + 1 - 2 * a) * 3 + (pw + 1 - 2 * b)) ? f[i][j] : 0.f;
+      acc = i == 0 ? v : acc + v;
+    }
+    d[j] = acc;
+  }
+  unpack_bf16x8(make_uint4(pack_bf16x2(d[0], d[1]), pack_bf16x2(d[2], d[3]), pack_bf16x2(d[4], d[5]), pack_bf16x2(d[6], d[7])),
+                d);
+}
+
+// psb_bn_bwd_reduce<true, true> with the dy load and the mask test replaced by pooled_grad8: the same CTA ranges, lanes and
+// per-thread pixel order, so every partial sum adds the same values in the same order
+__global__ void __launch_bounds__(BN_THREADS, 3) psb_bn_relu_maxpool_bwd_reduce(const __nv_bfloat16* __restrict__ dp,
+                                                                              const uint8_t* __restrict__ arg,
+                                                                              const __nv_bfloat16* __restrict__ x,
+                                                                              const float* __restrict__ mean,
+                                                                              const float* __restrict__ rstd,
+                                                                              float* __restrict__ part, BnGeom g, TailGeom t) {
+  extern __shared__ float smem[];
+  const int tx = threadIdx.x % g.groups, ty = threadIdx.x / g.groups;
+  float s[8], q[8], mu[8], rs[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    s[j] = q[j] = 0.f;
+    mu[j] = mean[tx * 8 + j];
+    rs[j] = rstd[tx * 8 + j];
+  }
+  const long long per_cta = (g.pixels + gridDim.x - 1) / gridDim.x;
+  const long long p0 = (long long)blockIdx.x * per_cta;
+  const long long p1 = p0 + per_cta < g.pixels ? p0 + per_cta : g.pixels;
+  if (ty < g.lanes) {
+    for (long long p = p0 + ty; p < p1; p += g.lanes) {   // min-blocks 3: 80 registers, no spills (92 without the cap)
+      float d[8], a[8];
+      ld8_stream(x + p * g.C + tx * 8, a);
+      pooled_grad8(dp, arg, (int)p, g.C, tx, t, d);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        s[j] += d[j];
+        q[j] = fmaf(d[j], (a[j] - mu[j]) * rs[j], q[j]);
+      }
+    }
+  }
+  reduce_lanes(smem, s, tx, ty, g, part + (size_t)blockIdx.x * 2 * g.C);
+  reduce_lanes(smem, q, tx, ty, g, part + (size_t)blockIdx.x * 2 * g.C + g.C);
+}
+
+// psb_bn_bwd_apply<false, true, true> with the same gather
+__global__ void __launch_bounds__(BN_THREADS) psb_bn_relu_maxpool_bwd_apply(const __nv_bfloat16* __restrict__ dp,
+                                                                             const uint8_t* __restrict__ arg,
+                                                                             const __nv_bfloat16* __restrict__ x,
+                                                                             const float* __restrict__ ca, const float* __restrict__ cb,
+                                                                             const float* __restrict__ cc, __nv_bfloat16* __restrict__ dx,
+                                                                             BnGeom g, TailGeom t) {
+  const int tx = threadIdx.x % g.groups, ty = threadIdx.x / g.groups;
+  if (ty >= g.lanes) return;
+  float a[8], b[8], c[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    a[j] = ca[tx * 8 + j];
+    b[j] = cb[tx * 8 + j];
+    c[j] = cc[tx * 8 + j];
+  }
+  const long long stride = (long long)gridDim.x * g.lanes;
+  for (long long p = (long long)blockIdx.x * g.lanes + ty; p < g.pixels; p += stride) {
+    const long long off = p * g.C + tx * 8;
+    float d[8], xv[8];
+    ld8_stream(x + off, xv);
+    pooled_grad8(dp, arg, (int)p, g.C, tx, t, d);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) xv[j] = fmaf(d[j], a[j], fmaf(xv[j], b[j], c[j]));
+    st8(dx + off, xv);
+  }
+}
+
 BnGeom geom(long long pixels, int C) {
   BnGeom g;
   g.pixels = pixels;
@@ -438,4 +608,47 @@ void psb_bn_backward(cudaStream_t s, const void* dy, const void* x, const void* 
     else PSB_APPLY(false, false, false);
   }
 #undef PSB_APPLY
+}
+
+// The ResNet stem tail, training (see psb_bn_relu_maxpool_fwd): finalize on the producer's sums, then BN + ReLU + 3x3/s2/p1
+// max-pool in one pass → pooled [N, H/2, W/2, C] and its 1-byte taps (255: the window routes no gradient).  H, W even.
+void psb_bn_relu_maxpool_forward_presummed(cudaStream_t s, const void* x, const void* gamma, const void* beta, const float* sums,
+                                           float* mean, float* rstd, float* scale, float* shift, float* running_mean,
+                                           float* running_var, int N, int H, int W, int C, float eps, float momentum, void* y,
+                                           void* arg) {
+  const long long pixels = (long long)N * H * W;
+  const BnGeom g = geom(pixels, C);
+  const TailGeom t{N, H, W, H / 2, W / 2};
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int rows = N * t.OH, grid = rows < sms * 16 ? rows : sms * 16;
+  psb_count_launch(2);
+  psb_bn_finalize<<<(C + FIN_CH - 1) / FIN_CH, FIN_THREADS, 0, s>>>(sums, 1, reinterpret_cast<const __nv_bfloat16*>(gamma),
+                                                   reinterpret_cast<const __nv_bfloat16*>(beta), mean, rstd, scale, shift,
+                                                   running_mean, running_var, C, pixels, eps, momentum);
+  psb_bn_relu_maxpool_fwd<<<grid, BN_THREADS, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(x), scale, shift,
+                                                       reinterpret_cast<__nv_bfloat16*>(y), reinterpret_cast<uint8_t*>(arg), g, t);
+}
+
+// Backward of the stem tail from the pooled gradient `dy` [N, H/2, W/2, C] and the forward's taps: reduce → finalize → apply,
+// as psb_bn_backward with relu and the mask, bit for bit.
+void psb_bn_relu_maxpool_backward(cudaStream_t s, const void* dy, const void* arg, const void* x, const void* gamma,
+                                  const float* mean, const float* rstd, float* part /*psb_bn_partial_floats*/, float* coef /*3C*/,
+                                  void* dx, void* dgamma, void* dbeta, int N, int H, int W, int C) {
+  const long long pixels = (long long)N * H * W;
+  const BnGeom g = geom(pixels, C);
+  const TailGeom t{N, H, W, H / 2, W / 2};
+  auto DY = reinterpret_cast<const __nv_bfloat16*>(dy);
+  auto A = reinterpret_cast<const uint8_t*>(arg);
+  auto X = reinterpret_cast<const __nv_bfloat16*>(x);
+  psb_count_launch(3);
+  const int rgrid = grid_for(pixels, g, REDUCE_MIN_ITERS);
+  psb_bn_relu_maxpool_bwd_reduce<<<rgrid, BN_THREADS, sizeof(float) * g.lanes * C, s>>>(DY, A, X, mean, rstd, part, g, t);
+  psb_bn_bwd_finalize<<<(C + FIN_CH - 1) / FIN_CH, FIN_THREADS, 0, s>>>(part, rgrid, reinterpret_cast<const __nv_bfloat16*>(gamma),
+                                                                         mean, rstd, coef, coef + C, coef + 2 * C,
+                                                                         reinterpret_cast<__nv_bfloat16*>(dgamma),
+                                                                         reinterpret_cast<__nv_bfloat16*>(dbeta), C, pixels);
+  psb_bn_relu_maxpool_bwd_apply<<<grid_for(pixels, g), BN_THREADS, 0, s>>>(DY, A, X, coef, coef + C, coef + 2 * C,
+                                                                           reinterpret_cast<__nv_bfloat16*>(dx), g, t);
 }

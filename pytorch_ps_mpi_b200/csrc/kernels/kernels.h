@@ -136,6 +136,16 @@ void psb_bn_forward_presummed(cudaStream_t s, const void* x, const void* res, co
 void psb_bn_backward(cudaStream_t s, const void* dy, const void* x, const void* y, const void* gamma, const float* mean,
                      const float* rstd, float* part, float* coef, void* dx, void* dres, void* dgamma, void* dbeta,
                      long long pixels, int C, int relu, const void* mask = nullptr /* the forward's ReLU bit mask, replaces y */);
+// ResNet stem tail (training, H and W even): BN + ReLU + 3x3/s2/p1 max-pool in one pass from the producer's sums → pooled y
+// [N, H/2, W/2, C] + 1-byte taps (255: routes no gradient); the backward takes the pooled gradient and the taps.
+// Bit-identical to psb_bn_forward_presummed → psb_maxpool3x3s2_forward → psb_maxpool3x3s2_backward → psb_bn_backward.
+void psb_bn_relu_maxpool_forward_presummed(cudaStream_t s, const void* x, const void* gamma, const void* beta, const float* sums,
+                                           float* mean, float* rstd, float* scale, float* shift, float* running_mean,
+                                           float* running_var, int N, int H, int W, int C, float eps, float momentum, void* y,
+                                           void* arg);
+void psb_bn_relu_maxpool_backward(cudaStream_t s, const void* dy, const void* arg, const void* x, const void* gamma,
+                                  const float* mean, const float* rstd, float* part, float* coef, void* dx, void* dgamma,
+                                  void* dbeta, int N, int H, int W, int C);
 
 // pool_kernels.cu — channels-last bf16 3x3/s2/p1 max pooling
 void psb_maxpool3x3s2_forward(cudaStream_t s, const void* x, void* y, void* arg, int N, int H, int W, int C);

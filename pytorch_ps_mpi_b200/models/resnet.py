@@ -21,6 +21,9 @@ from ..ops.stem import STEM_K, STEM_STRIDES, stem_conv, stem_conv_fused, stem_fu
 # statistics in its epilogue (csrc/kernels/stem_kernels.cu) instead of im2col + GEMM + statistics pass.
 # PSB200_STEM=im2col restores the round-1 path.
 _FUSED_STEM = os.environ.get("PSB200_STEM", "fused").lower() != "im2col"
+# With the fused stem, BN1 + ReLU + max-pool run as one forward kernel and a two-pass backward that never materialise the
+# 112x112 activation or its gradient (ops/batchnorm.py: forward_maxpool); PSB200_STEM_TAIL=unfused keeps the separate kernels.
+_FUSED_TAIL = os.environ.get("PSB200_STEM_TAIL", "fused").lower() != "unfused"
 
 def _conv3x3(i, o, stride=1):
     return nn.Conv2d(i, o, 3, stride, 1, bias=False)
@@ -134,6 +137,8 @@ class ResNet(nn.Module):
 
     def _tail(self, y, sums=None):
         """BN1 + ReLU + max-pool after the stem convolution."""
+        if sums is not None and _FUSED_TAIL and self.bn1.maxpool_ok(y):
+            return self.bn1.forward_maxpool(y, sums)
         return self.maxpool(self.bn1(y, sums=sums) if sums is not None else self.bn1(y))
 
     def attach(self, optimizer) -> "ResNet":

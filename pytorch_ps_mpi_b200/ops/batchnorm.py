@@ -47,6 +47,29 @@ class _FusedBN(torch.autograd.Function):
         return dx, (dres if ctx.has_res else None), dgamma, dbeta, None, None, None, None, None, None, None
 
 
+class _FusedBNMaxPool(torch.autograd.Function):
+    """Training BN (sums from the producer) + ReLU + 3x3/s2/p1 max-pool: the ResNet stem tail without its full-resolution
+    output or gradient.  Saves x and the pooled taps, no ReLU mask."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, running_mean, running_var, eps, momentum, sums):
+        y, mean, rstd, arg = ext.cuda().bn_forward_presummed(x, None, gamma, beta, running_mean, running_var, eps, momentum, True,
+                                                             sums, pool=True)
+        ctx.save_for_backward(x, arg, gamma, mean, rstd)
+        ctx.gout = (getattr(gamma, "ps_grad_out", None), getattr(beta, "ps_grad_out", None))
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, arg, gamma, mean, rstd = ctx.saved_tensors
+        if not dy.is_contiguous(memory_format=torch.channels_last):
+            dy = dy.contiguous(memory_format=torch.channels_last)
+        og = ctx.gout[0]() if ctx.gout[0] is not None else None
+        ob = ctx.gout[1]() if ctx.gout[1] is not None else None
+        dx, _, dgamma, dbeta = ext.cuda().bn_backward(dy, x, x, gamma, mean, rstd, True, False, og, ob, pool_arg=arg)
+        return dx, dgamma, dbeta, None, None, None, None, None
+
+
 def _kernel_ok(x: torch.Tensor, res: Optional[torch.Tensor], weight) -> bool:
     return (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and weight is not None
             and weight.dtype == torch.bfloat16 and x.shape[1] % 8 == 0 and x.shape[1] <= 2048
@@ -88,15 +111,30 @@ class FusedBatchNormAct2d(nn.BatchNorm2d):
                 setattr(self, name, b.float())
         return self
 
+    def _count_batch(self):
+        if self.training and self.num_batches_tracked is not None:
+            if self.momentum is None:
+                self.num_batches_tracked.add_(1)
+            else:
+                self._nbt_pending += 1
+
+    def maxpool_ok(self, x: torch.Tensor) -> bool:
+        """Whether :meth:`forward_maxpool` covers ``x``: training, ReLU, the kernels' layout and even H and W."""
+        return (self.training and self.relu and self.running_mean is not None and _kernel_ok(x, None, self.weight)
+                and x.shape[2] % 2 == 0 and x.shape[3] % 2 == 0)
+
+    def forward_maxpool(self, x: torch.Tensor, sums: torch.Tensor) -> torch.Tensor:
+        """``max_pool2d(self(x, sums=sums), 3, 2, 1)`` in one pass forward and two backward, bit for bit (needs
+        :meth:`maxpool_ok`)."""
+        self._count_batch()
+        return _FusedBNMaxPool.apply(x, self.weight, self.bias, self.running_mean, self.running_var, self.eps,
+                                     self.momentum if self.momentum is not None else 0.1, sums)
+
     def forward(self, x: torch.Tensor, residual: Optional[torch.Tensor] = None,
                 sums: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``sums``: fp32 ``[2C]`` = Σx | Σx² over N·H·W already computed by the producer of ``x``."""
         if _kernel_ok(x, residual, self.weight) and (self.training or self.running_mean is not None):
-            if self.training and self.num_batches_tracked is not None:
-                if self.momentum is None:
-                    self.num_batches_tracked.add_(1)
-                else:
-                    self._nbt_pending += 1
+            self._count_batch()
             return _FusedBN.apply(x, residual, self.weight, self.bias, self.running_mean, self.running_var,
                                   self.eps, self.momentum if self.momentum is not None else 0.1, self.relu, self.training,
                                   sums)
