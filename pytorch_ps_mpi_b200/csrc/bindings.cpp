@@ -121,14 +121,35 @@ struct UpdatePlan {
   }
 };
 
+// Fill a.batch with grads[base, base + PSB_ENCODE_MAX) (one launch) and a.grad_dt with the gradients' dtype.
+void fill_batch(EncodeArgs& a, const char* what, const std::vector<at::Tensor>& grads, const std::vector<int>& first_tile,
+                const std::vector<int>& ntiles, const std::vector<int>& param_idx, size_t base) {
+  const std::string w(what);
+  const int m = (int)std::min<size_t>(PSB_ENCODE_MAX, grads.size() - base);
+  a.grad_dt = dt_code(grads[0].scalar_type());
+  a.batch.n = m;
+  a.batch.cum[0] = 0;
+  for (int i = 0; i < m; ++i) {
+    const at::Tensor& g = grads[base + i];
+    if (!g.is_cuda() || !g.is_non_overlapping_and_dense()) throw std::runtime_error(w + ": gradients must be dense CUDA tensors");
+    if (dt_code(g.scalar_type()) != a.grad_dt) throw std::runtime_error(w + ": mixed gradient dtypes in one bucket");
+    if (reinterpret_cast<uintptr_t>(g.data_ptr()) % 16 != 0) throw std::runtime_error(w + ": gradient not 16-byte aligned");
+    a.batch.src[i] = g.data_ptr();
+    a.batch.first_tile[i] = first_tile[base + i];
+    a.batch.param[i] = param_idx[base + i];
+    a.batch.cum[i + 1] = a.batch.cum[i] + ntiles[base + i];
+  }
+}
+
 void encode(int kind, int wire, const std::vector<at::Tensor>& grads, const std::vector<int>& first_tile,
             const std::vector<int>& ntiles, const std::vector<int>& param_idx, uint64_t tiles_ptr, uint64_t wire_ptr,
             uint64_t scales_ptr, uint64_t amax_ptr, uint64_t residual_ptr, int bytes_per_tile, int cap, double ratio,
             const std::vector<uint64_t>& sig_targets, int sig_slot, uint64_t sig_value, uint64_t sig_counter,
-            uint64_t stream, uint64_t seed, uint32_t step, uint32_t rank, int levels) {
+            uint64_t stream, uint64_t seed, uint32_t step, uint32_t rank, int levels, bool keep_leftover) {
   const size_t n = grads.size();
   if (first_tile.size() != n || ntiles.size() != n || param_idx.size() != n) throw std::runtime_error("encode: length mismatch");
   if (n == 0) return;
+  if (residual_ptr % 16 != 0) throw std::runtime_error("encode: carry not 16-byte aligned");
   cudaStream_t s = pick_stream(stream);
   EncodeArgs a{};
   a.tiles = reinterpret_cast<const TileInfo*>(tiles_ptr);
@@ -136,27 +157,15 @@ void encode(int kind, int wire, const std::vector<at::Tensor>& grads, const std:
   a.scales = reinterpret_cast<float*>(scales_ptr);
   a.amax_bits = reinterpret_cast<uint32_t*>(amax_ptr);
   a.residual = reinterpret_cast<float*>(residual_ptr);
+  a.drop_leftover = keep_leftover ? 0 : 1;
   a.bytes_per_tile = bytes_per_tile;
   a.cap = cap;
   a.ratio = ratio;
-  a.grad_dt = dt_code(grads[0].scalar_type());
   a.seed = seed, a.step = step, a.rank = rank, a.levels = levels;
   if (kind == KIND_QSGD && (levels < 1 || levels > (wire == WIRE_I4 ? 7 : 127)))
     throw std::runtime_error("encode: QSGD levels out of range for the wire");
   for (size_t base = 0; base < n; base += PSB_ENCODE_MAX) {
-    const int m = (int)std::min<size_t>(PSB_ENCODE_MAX, n - base);
-    a.batch.n = m;
-    a.batch.cum[0] = 0;
-    for (int i = 0; i < m; ++i) {
-      const at::Tensor& g = grads[base + i];
-      if (!g.is_cuda() || !g.is_non_overlapping_and_dense()) throw std::runtime_error("encode: gradients must be dense CUDA tensors");
-      if (dt_code(g.scalar_type()) != a.grad_dt) throw std::runtime_error("encode: mixed gradient dtypes in one bucket");
-      if (reinterpret_cast<uintptr_t>(g.data_ptr()) % 16 != 0) throw std::runtime_error("encode: gradient not 16-byte aligned");
-      a.batch.src[i] = g.data_ptr();
-      a.batch.first_tile[i] = first_tile[base + i];
-      a.batch.param[i] = param_idx[base + i];
-      a.batch.cum[i + 1] = a.batch.cum[i] + ntiles[base + i];
-    }
+    fill_batch(a, "encode", grads, first_tile, ntiles, param_idx, base);
     if (kind == KIND_SCALED) {
       psb_launch_absmax(s, a);
       check_launch("psb_absmax_kernel launch");
@@ -172,6 +181,23 @@ void encode(int kind, int wire, const std::vector<at::Tensor>& grads, const std:
     }
     psb_launch_encode(s, kind, wire, a);
     check_launch("psb_encode_kernel launch");
+  }
+}
+
+// Gradient accumulation: carry[tile * TILE + i] += g[i] in fp32 for every gradient (their arena tiles), in list order.
+void accumulate(const std::vector<at::Tensor>& grads, const std::vector<int>& first_tile, const std::vector<int>& ntiles,
+                const std::vector<int>& param_idx, uint64_t tiles_ptr, uint64_t carry_ptr, uint64_t stream) {
+  const size_t n = grads.size();
+  if (first_tile.size() != n || ntiles.size() != n || param_idx.size() != n) throw std::runtime_error("accumulate: length mismatch");
+  if (n == 0) return;
+  if (carry_ptr == 0 || carry_ptr % 16 != 0) throw std::runtime_error("accumulate: carry missing or not 16-byte aligned");
+  EncodeArgs a{};
+  a.tiles = reinterpret_cast<const TileInfo*>(tiles_ptr);
+  a.residual = reinterpret_cast<float*>(carry_ptr);
+  for (size_t base = 0; base < n; base += PSB_ENCODE_MAX) {
+    fill_batch(a, "accumulate", grads, first_tile, ntiles, param_idx, base);
+    psb_launch_accumulate(pick_stream(stream), a);
+    check_launch("psb_accumulate_kernel launch");
   }
 }
 
@@ -305,7 +331,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("residual_ptr"), py::arg("bytes_per_tile"), py::arg("cap"), py::arg("ratio"),
         py::arg("sig_targets") = std::vector<uint64_t>{}, py::arg("sig_slot") = 0, py::arg("sig_value") = 0,
         py::arg("sig_counter") = 0, py::arg("stream") = 0, py::arg("seed") = 0, py::arg("step") = 0, py::arg("rank") = 0,
-        py::arg("levels") = 0);
+        py::arg("levels") = 0, py::arg("keep_leftover") = true);
+  m.def("accumulate", &accumulate, py::arg("grads"), py::arg("first_tile"), py::arg("ntiles"), py::arg("param_idx"),
+        py::arg("tiles_ptr"), py::arg("carry_ptr"), py::arg("stream") = 0,
+        "gradient accumulation: carry (fp32, arena-shaped) += each gradient, one launch per PSB_ENCODE_MAX gradients");
   m.def("signal", &signal, py::arg("targets"), py::arg("slot"), py::arg("value"), py::arg("extra_slot") = -1,
         py::arg("extra_value") = 0, py::arg("stream") = 0, py::arg("version_local") = 0, py::arg("version_slot") = 0);
   m.def("wait_flags", &wait_flags, py::arg("signal_local"), py::arg("slot0"), py::arg("mask"), py::arg("want"),

@@ -22,7 +22,8 @@ struct EncodeArgs {
   void* wire;            // local wire arena
   float* scales;         // local per-parameter scale table (KIND_SCALED)
   uint32_t* amax_bits;   // per-parameter abs-max scratch (float bits, atomicMax)
-  float* residual;       // error-feedback residual (flat fp32) or nullptr
+  float* residual;       // fp32 arena-shaped carry added to the gradient before encoding (top-k error-feedback residual, or
+                         // the gradient-accumulation sum), or nullptr; left zero after encoding, or the top-k leftover
   int32_t bytes_per_tile;
   int32_t cap;           // top-k entries per tile
   double ratio;
@@ -39,6 +40,8 @@ struct EncodeArgs {
   uint32_t step;
   uint32_t rank;
   int32_t levels;
+  // KIND_TOPK with a carry: leave it zero instead of keeping the leftover (accumulation without error feedback)
+  int32_t drop_leftover;
 };
 
 struct UpdateArgs {
@@ -84,6 +87,9 @@ struct UpdateArgs {
 
 void psb_launch_absmax(cudaStream_t s, const EncodeArgs& a);
 void psb_launch_encode(cudaStream_t s, int kind, int wire, const EncodeArgs& a);
+// gradient accumulation: residual[tile * PSB_TILE + i] += g[i] (fp32) for every tile of the batch; reads the gradients as the
+// encode does (batch, tiles, grad_dt, residual are the only fields used)
+void psb_launch_accumulate(cudaStream_t s, const EncodeArgs& a);
 void psb_launch_update(cudaStream_t s, int kind, int wire, int opt, const UpdateArgs& a, int grid);
 void psb_launch_signal(cudaStream_t s, uint64_t* const* targets, int ntargets, int slot, uint64_t value,
                        uint64_t* extra_slot_base, int extra_slot, uint64_t extra_value, uint64_t* version_local = nullptr,

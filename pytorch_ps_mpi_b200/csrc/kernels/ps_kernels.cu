@@ -80,9 +80,38 @@ __device__ __forceinline__ void load_grad8(const EncodeArgs& a, int entry, const
   }
 }
 
+// this thread's 8 elements of the fp32 carry (arena-shaped: element i of tile t at t * PSB_TILE + i)
+__device__ __forceinline__ float4* carry8(const EncodeArgs& a, int tile) {
+  return reinterpret_cast<float4*>(a.residual + (size_t)tile * PSB_TILE + threadIdx.x * PSB_EPT);
+}
+
+__device__ __forceinline__ void add_carry8(const EncodeArgs& a, int tile, float* g) {
+  const float4* r = carry8(a, tile);
+  const float4 r0 = r[0], r1 = r[1];
+  g[0] += r0.x, g[1] += r0.y, g[2] += r0.z, g[3] += r0.w;
+  g[4] += r1.x, g[5] += r1.y, g[6] += r1.z, g[7] += r1.w;
+}
+
+// ------------------------------------------------------------------------------------------
+// gradient accumulation (no_sync): carry += gradient in fp32, one add per element, one launch per bucket; padding lanes add 0
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(PSB_THREADS) psb_accumulate_kernel(const __grid_constant__ EncodeArgs a) {
+  int entry, tile;
+  locate(a.batch, blockIdx.x, entry, tile);
+  const TileInfo ti = a.tiles[tile];
+  float g[PSB_EPT];
+  load_grad8(a, entry, ti, tile, g);
+  float4* r = carry8(a, tile);
+  const float4 r0 = r[0], r1 = r[1];
+  r[0] = make_float4(r0.x + g[0], r0.y + g[1], r0.z + g[2], r0.w + g[3]);
+  r[1] = make_float4(r1.x + g[4], r1.y + g[5], r1.z + g[6], r1.w + g[7]);
+}
+
 // ------------------------------------------------------------------------------------------
 // abs-max pre-pass for Scale codings: one atomicMax per tile into amax_bits[param]
 // ------------------------------------------------------------------------------------------
+// CARRY: the instantiation for a.residual != nullptr (the plain pass keeps its registers)
+template <bool CARRY>
 __global__ void __launch_bounds__(PSB_THREADS) psb_absmax_kernel(const __grid_constant__ EncodeArgs a) {
   __shared__ float red[PSB_THREADS / 32];
   int entry, tile;
@@ -90,6 +119,7 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_absmax_kernel(const __grid_co
   const TileInfo ti = a.tiles[tile];
   float g[PSB_EPT];
   load_grad8(a, entry, ti, tile, g);
+  if constexpr (CARRY) add_carry8(a, tile, g);   // the abs-max of what the encode will see
   float m = 0.f;
 #pragma unroll
   for (int j = 0; j < PSB_EPT; ++j) m = fmaxf(m, isfinite(g[j]) ? fabsf(g[j]) : 0.f);   // amax over finite elements only
@@ -211,8 +241,11 @@ __device__ __forceinline__ void unpack_i4x8(uint32_t w, float* f) {
   }
 }
 
-template <int KIND, int WIRE>
+// CARRY: the instantiation for a.residual != nullptr, so the plain encode keeps its registers.  Top-k always has CARRY = false
+// and tests a.residual at run time: its error-feedback residual is older than gradient accumulation.
+template <int KIND, int WIRE, bool CARRY>
 __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_constant__ EncodeArgs a) {
+  const bool carry = KIND == KIND_TOPK ? a.residual != nullptr : CARRY;
   int entry, tile;
   locate(a.batch, blockIdx.x, entry, tile);
   const TileInfo ti = a.tiles[tile];
@@ -220,6 +253,7 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_co
   uint8_t* wire_tile = reinterpret_cast<uint8_t*>(a.wire) + (size_t)tile * a.bytes_per_tile;
   float g[PSB_EPT];
   load_grad8(a, entry, ti, tile, g);
+  if (carry) add_carry8(a, tile, g);
 
   if constexpr (KIND == KIND_DENSE) {
     store_dense<WIRE>(wire_tile, g, a.grad_dt != DT_F16);
@@ -238,13 +272,6 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_co
     __shared__ uint32_t hist[256];
     __shared__ uint32_t warp_tot[PSB_THREADS / 32];
     __shared__ uint32_t s_prefix, s_k;
-    const size_t e0 = (size_t)tile * PSB_TILE + tid * PSB_EPT;
-    if (a.residual) {
-      const float4* r = reinterpret_cast<const float4*>(a.residual + e0);
-      float4 r0 = r[0], r1 = r[1];
-      g[0] += r0.x, g[1] += r0.y, g[2] += r0.z, g[3] += r0.w;
-      g[4] += r1.x, g[5] += r1.y, g[6] += r1.z, g[7] += r1.w;
-    }
     uint32_t key[PSB_EPT];
 #pragma unroll
     for (int j = 0; j < PSB_EPT; ++j) key[j] = (tid * PSB_EPT + j < ti.valid) ? (__float_as_uint(g[j]) & 0x7fffffffu) : 0u;
@@ -332,11 +359,12 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_co
       if constexpr (WIRE == WIRE_BF16) reinterpret_cast<uint32_t*>(wire_tile)[p] = (uint32_t)PSB_TILE << 16;
       else reinterpret_cast<uint2*>(wire_tile)[p] = make_uint2(PSB_TILE, 0u);
     }
-    if (a.residual) {
-      float4* r = reinterpret_cast<float4*>(a.residual + e0);
-      r[0] = make_float4(g[0], g[1], g[2], g[3]);
-      r[1] = make_float4(g[4], g[5], g[6], g[7]);
-    }
+  }
+  if (carry) {   // the carry is consumed: error-feedback top-k keeps what the wire did not take, everything else zero
+    const bool keep = KIND == KIND_TOPK && !a.drop_leftover;
+    float4* r = carry8(a, tile);
+    r[0] = keep ? make_float4(g[0], g[1], g[2], g[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+    r[1] = keep ? make_float4(g[4], g[5], g[6], g[7]) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
 
   // ---- fused flag raise (last encode launch of the step): the last CTA to finish publishes GRAD_READY ----
@@ -963,7 +991,16 @@ unsigned long long psb_launch_count() { return g_psb_launches.load(std::memory_o
 void psb_launch_absmax(cudaStream_t s, const EncodeArgs& a) {
   const int ctas = a.batch.cum[a.batch.n];
   if (ctas > 0) {
-    psb_absmax_kernel<<<ctas, PSB_THREADS, 0, s>>>(a);
+    if (a.residual) psb_absmax_kernel<true><<<ctas, PSB_THREADS, 0, s>>>(a);
+    else psb_absmax_kernel<false><<<ctas, PSB_THREADS, 0, s>>>(a);
+    psb_count_launch(1);
+  }
+}
+
+void psb_launch_accumulate(cudaStream_t s, const EncodeArgs& a) {
+  const int ctas = a.batch.cum[a.batch.n];
+  if (ctas > 0) {
+    psb_accumulate_kernel<<<ctas, PSB_THREADS, 0, s>>>(a);
     psb_count_launch(1);
   }
 }
@@ -972,10 +1009,16 @@ void psb_launch_encode(cudaStream_t s, int kind, int wire, const EncodeArgs& a) 
   const int ctas = a.batch.cum[a.batch.n];
   if (ctas <= 0) return;
   psb_count_launch(1);
-#define ENC(K, W)                                            \
-  if (kind == K && wire == W) {                              \
-    psb_encode_kernel<K, W><<<ctas, PSB_THREADS, 0, s>>>(a); \
-    return;                                                  \
+#define ENC(K, W)                                                     \
+  if (kind == K && wire == W) {                                       \
+    if constexpr (K != KIND_TOPK) {                                   \
+      if (a.residual) {                                               \
+        psb_encode_kernel<K, W, true><<<ctas, PSB_THREADS, 0, s>>>(a); \
+        return;                                                       \
+      }                                                               \
+    }                                                                 \
+    psb_encode_kernel<K, W, false><<<ctas, PSB_THREADS, 0, s>>>(a);   \
+    return;                                                           \
   }
   ENC(KIND_DENSE, WIRE_F32) ENC(KIND_DENSE, WIRE_BF16) ENC(KIND_DENSE, WIRE_F16) ENC(KIND_DENSE, WIRE_E4M3)
   ENC(KIND_DENSE, WIRE_E5M2) ENC(KIND_SCALED, WIRE_I8) ENC(KIND_SCALED, WIRE_E4M3) ENC(KIND_SCALED, WIRE_E5M2)

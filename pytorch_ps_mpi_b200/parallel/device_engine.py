@@ -36,7 +36,7 @@ import torch
 from .. import runtime
 from ..codings import KIND_DENSE, KIND_QSGD, KIND_SCALED, KIND_TOPK, TILE, WIRE_BF16, WIRE_F16, WIRE_F32, wire_code_of
 from ..ops import ext
-from ..utils.misc import CudaStepTimer
+from ..utils.misc import CudaStepTimer, MicroBatchCounter
 from .layout import FlatLayout
 from .symmetric import SymmetricArena
 
@@ -141,6 +141,14 @@ class DeviceEngine:
         self.residual = None
         if self.kind == KIND_TOPK and self.spec.error_feedback:
             self.residual = torch.zeros(n_pad, dtype=torch.float32, device=self.device)
+        # gradient accumulation (MPI_PS.no_sync): micro-batch gradients are summed in fp32 into `carry` (arena-shaped, allocated on
+        # first use; error-feedback top-k sums into its residual) by accumulate launches on the compute stream; the step's encode
+        # adds the carry to the last gradient (or to `_zeros` for a parameter that fired only inside no_sync) and zeroes it
+        self.carry = None
+        self._carry_ptr = 0
+        self._zeros = None
+        self._no_sync = False
+        self._mb = MicroBatchCounter()
         self.master = self.buf0 = self.buf1 = self.buf2 = None
         if self.is_server:
             if self.dtype != torch.float32 and master_fp32:
@@ -323,6 +331,11 @@ class DeviceEngine:
         self._chunk_items: List[list] = [[] for _ in self.chunks]
         self._chunk_left = [len(c) for c in self.chunks]
         self._next_chunk = 0
+        self._carried: set = set()           # parameters with a contribution in the carry this step
+        self._acc_items: List[list] = [[] for _ in self.chunks]   # accumulates not yet launched, per chunk
+        self._acc_left = [len(c) for c in self.chunks]           # per chunk: parameters yet to fire in this micro-batch
+        self._acc_waited = False
+        self._mb.reset()
 
     def _progress(self, epoch: int, chunk: int) -> int:
         """Monotone GRAD_READY value meaning "chunks 0..chunk of step ``epoch`` are in my wire arena"."""
@@ -405,8 +418,8 @@ class DeviceEngine:
         ``psb_encode_kernel`` copy: ``on_grad`` recognises the pointer and only counts the parameter as arrived.  Safe in
         ``mode='ps'`` only: a worker's backward starts after it observed PARAMS_READY (the server finished reading the
         previous wire tiles); in ``allgather`` mode peers may still be reading them (CONSUMED is awaited on the comm stream)."""
-        if not self._direct_ok or self._closed:
-            return None
+        if not self._direct_ok or self._closed or self.accumulating:
+            return None                      # (an accumulated step encodes from the carry)
         sl = self.layout.by_id.get(id(param))
         if sl is None:
             return None
@@ -436,9 +449,17 @@ class DeviceEngine:
             elif g.stride() != param.stride() or g.data_ptr() % 16:
                 # the arena is in the parameter's physical order: bring the gradient into it
                 g = torch.empty_strided(param.shape, param.stride(), dtype=g.dtype, device=g.device).copy_(g)
-        if s.index in self._fired:           # gradient accumulation: later micro-batches add up
-            raise RuntimeError(f"parameter {name!r} produced two gradients before step(); "
-                               "call step() after every backward (the reference encodes per backward)")
+        if self._mb.fire(s.index):           # a new backward pass: the previous one's gradients are summed first
+            self._flush_accumulate()
+            self._acc_left = [len(c) for c in self.chunks]
+        if s.index in self._fired:
+            raise RuntimeError(f"parameter {name!r} produced two gradients before step(); call step() after every backward, "
+                               "or run the earlier backwards inside opt.no_sync() to accumulate them")
+        if self._no_sync:
+            self._accumulate(s, g, param)
+            return
+        if self._carried:
+            self._drop_wire_alias(param)
         self._fired.add(s.index)
         k = self._chunk_of[s.index]
         self._chunk_left[k] -= 1
@@ -454,6 +475,73 @@ class DeviceEngine:
             self._chunk_items[k].append((s, g))
         while self._next_chunk < self.nchunks and self._chunk_left[self._next_chunk] == 0:
             self._flush_chunk(self._next_chunk)
+
+    # ------------------------------------------------------------------------- accumulation
+    @property
+    def accumulating(self) -> bool:
+        """Inside ``no_sync()``, or the carry holds gradients the next ``step()`` has not sent yet."""
+        return self._no_sync or bool(self._carried)
+
+    def begin_no_sync(self):
+        if self.mode == "async" and self.size > 1 and self.rank == 0:
+            return                           # the dedicated server runs no backward
+        if self.carry is None:
+            L = self.layout
+            self.carry = self.residual if self.residual is not None else \
+                torch.zeros(L.numel_padded, dtype=torch.float32, device=self.device)
+            self._carry_ptr = self.carry.data_ptr()
+            self._zeros = torch.zeros(max(s.numel for s in L.slots), dtype=self.dtype, device=self.device)
+        self._no_sync = True
+        self._mb.cut()
+
+    def end_no_sync(self):
+        self._flush_accumulate()
+        self._no_sync = False
+        self._mb.cut()
+
+    def _drop_wire_alias(self, param):
+        """After a direct-placement step ``param.grad`` can still view the wire arena (``zero_grad(set_to_none=False)``):
+        AccumulateGrad would add this gradient into a wire tile the server may be reading.  Drop it: the gradient is assigned."""
+        g = param.grad
+        if g is not None and self._direct_ok and 0 <= g.data_ptr() - self._wire_ptr < self.wire_arena.numel():
+            param.grad = None
+
+    def _accumulate(self, s, g, param):
+        """A gradient inside ``no_sync()``: queue it for the carry; each chunk is summed once all its parameters fired."""
+        self._drop_wire_alias(param)
+        self._carried.add(s.index)
+        k = self._chunk_of[s.index]
+        self._acc_items[k].append((s, g))
+        self._acc_left[k] -= 1
+        if self._acc_left[k] == 0:
+            self._flush_accumulate(k)
+
+    def _flush_accumulate(self, k: Optional[int] = None):
+        """carry += the queued gradients (of chunk ``k``, or all), on the compute stream: the gradients need not outlive it."""
+        items = []
+        for j in (range(self.nchunks) if k is None else (k,)):
+            items += self._acc_items[j]
+            self._acc_items[j] = []
+        if not items:
+            return
+        if not self._acc_waited:
+            self._acc_waited = True
+            if self._prev_done is not None:  # the last step's encode zeroed (or wrote the leftover into) the carry on the comm stream
+                torch.cuda.current_stream(self.device).wait_event(self._prev_done)
+        self.m.accumulate([g for _, g in items], [s.first_tile for s, _ in items], [s.ntiles for s, _ in items],
+                          [s.index for s, _ in items], self._tiles_ptr, self._carry_ptr)
+        self.launches += (len(items) + 63) // 64
+
+    def _close_accumulation(self):
+        """step(): sum what is still queued; parameters that fired only inside no_sync() are encoded from the carry alone."""
+        self._flush_accumulate()
+        for i in sorted(self._carried - self._fired):
+            s = self.layout.slots[i]
+            k = self._chunk_of[i]
+            self._fired.add(i)
+            self._chunk_left[k] -= 1
+            self._raw_bytes += s.numel * self.psz
+            self._chunk_items[k].append((s, self._zeros[: s.numel]))
 
     def _event(self, timing: bool = False):
         """A pooled CUDA event (creating one costs more than recording one)."""
@@ -498,14 +586,17 @@ class DeviceEngine:
         items, self._chunk_items[k] = self._chunk_items[k], []
         if items:
             grads = [g for _, g in items]
-            qsgd = dict(seed=self.spec.seed, step=self._qsgd_step & 0xFFFFFFFF, rank=self.rank,
-                        levels=self.spec.levels) if self.kind == KIND_QSGD else {}
+            kw = dict(seed=self.spec.seed, step=self._qsgd_step & 0xFFFFFFFF, rank=self.rank,
+                      levels=self.spec.levels) if self.kind == KIND_QSGD else {}
+            if self._carried:                 # an accumulated step: the encode adds the carry and zeroes it
+                kw["keep_leftover"] = self.residual is not None
             m.encode(self.kind, self.wire, grads, [s.first_tile for s, _ in items],
                      [s.ntiles for s, _ in items], [s.index for s, _ in items],
-                     self._tiles_ptr, self._wire_ptr, self._scales_ptr, self._amax_ptr, self._residual_ptr,
+                     self._tiles_ptr, self._wire_ptr, self._scales_ptr, self._amax_ptr,
+                     self._carry_ptr if self._carried else self._residual_ptr,
                      self.bpt, self.cap, self._ratio,
                      *((sig[0], sig[1], sig[2], self._sigctr_ptr) if sig else ([], 0, 0, 0)),
-                     csh, **qsgd)
+                     csh, **kw)
             nb = (len(items) + 63) // 64
             self.launches += nb * (2 if self.kind == KIND_SCALED else 1)
             self._keep.extend(grads)
@@ -657,6 +748,7 @@ class DeviceEngine:
                 "iallgather_prepare_time": 0.0, "isend_time": 0.0}
         if self.mode == "async" and self.size > 1:
             return self._step_async(data)
+        self._close_accumulation()
         epoch = self._epoch + 1
         m, cs = self.m, self.comm_stream
         prof = self._prof.enabled
@@ -702,6 +794,7 @@ class DeviceEngine:
         wire_bytes = sum(L.slots[i].ntiles for i in self._fired) * self.bpt if self._fired else 0
         data["packaged_bytes"] = wire_bytes / nfired
         data["engine"] = "device"
+        data["micro_batches"] = self._mb.n
         self._epoch += 1
         self._qsgd_step += 1
         if len(self._fired) != L.nparams:
@@ -751,9 +844,12 @@ class DeviceEngine:
             self.counters.zero_()
             self._consumed.zero_()
             self._select_out.zero_()
+            if self.carry is not None:
+                self.carry.zero_()            # an open accumulation is dropped
         self._err_host.zero_()
         self._err_event = None
         self._epoch = 0
+        self._no_sync = False
         self._start_step()
         self._keep_prev = []
         self._prev_done = None
@@ -805,6 +901,7 @@ class DeviceEngine:
         cs = self.comm_stream
         cur = torch.cuda.current_stream(self.device)
         if self.rank != 0:
+            self._close_accumulation()
             epoch = self._epoch + 1
             ev = self._event()
             ev.record(cur)

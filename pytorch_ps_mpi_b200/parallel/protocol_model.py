@@ -36,7 +36,7 @@ import sys
 from dataclasses import dataclass, field
 from typing import Dict, FrozenSet, Iterable, List, Optional, Sequence, Tuple
 
-__all__ = ["Violation", "Result", "Model", "build_ps", "build_ps_unpipelined", "build_allgather", "build_allgather_unpipelined", "build_async", "build_stem_pipeline", "build_stem_wgrad_pipeline",
+__all__ = ["Violation", "Result", "Model", "build_ps", "build_ps_unpipelined", "build_allgather", "build_allgather_unpipelined", "build_async", "build_ps_accumulate", "build_stem_pipeline", "build_stem_wgrad_pipeline",
            "check", "MODES"]
 
 DONE = 1 << 62          # device_engine._DONE_EPOCH / PSB_DONE_EPOCH
@@ -554,6 +554,61 @@ def build_ps(n: int, epochs: int, drop: Optional[str] = None) -> Model:
     return m
 
 
+def build_ps_accumulate(n: int, epochs: int, drop: Optional[str] = None) -> Model:
+    """``mode='ps'`` (pipelined, two chunks) with gradient accumulation: every step is one backward inside ``no_sync()`` and a
+    final one.  The carry of each chunk is a resource: the no_sync backward's gradients are added into it by an accumulate
+    launch on the COMPUTE stream (``DeviceEngine._flush_accumulate``; the first of a step waits for the comm stream's ``done``
+    of the previous step, whose encodes zeroed the carry); the final backward's encode on the comm stream reads and zeroes it.
+    After a direct-placement step ``param.grad`` may still view the wire tile; the hook drops it, so AccumulateGrad assigns the
+    final gradient instead of adding it into the tile after the encode wrote it.
+
+    ``drop``: ``'prev_done'`` (the first accumulate does not wait for the previous step's encodes), ``'alias'`` (the hook keeps a
+    ``param.grad`` that views the wire tile: AccumulateGrad adds into it after the final encode) — each must be caught."""
+    m = Model()
+    prog = lambda e, c: (e - 1) * 2 + c + 1      # noqa: E731
+    for r in range(n):
+        comp, comm = [], []
+        for e in range(1, epochs + 1):
+            if r != 0 and e > 1:
+                comp.append(("wait", ("PARAMS_READY", r), e - 1))
+            if r == 0 and e > 1:
+                comp.append(("wev", ("done", 0, e - 1)))
+            # micro-batch 1, inside no_sync(): its gradients are fresh tensors, summed into the carry on the compute stream
+            comp.append(("acq", [(("paramsA", r), "r", e - 1), (("paramsB", r), "r", e - 1), (("accg", r, e), "w", None)]))
+            comp.append(("rel", [(("paramsA", r), "r", None), (("paramsB", r), "r", None), (("accg", r, e), "w", e)]))
+            if e > 1 and drop != "prev_done":
+                comp.append(("wev", ("done", r, e - 1)))
+            comp.append(("acq", [(("accg", r, e), "r", e), (("carryA", r), "w", 2 * e - 2), (("carryB", r), "w", 2 * e - 2)]))
+            comp.append(("rel", [(("accg", r, e), "r", None), (("carryA", r), "w", 2 * e - 1), (("carryB", r), "w", 2 * e - 1)]))
+            # the final backward: the pipelined chunks, each encoded with its carry
+            _backward_chunks(m, r, e, comp, prev_done=(r != 0))
+            if drop == "alias" and r != 0:
+                # AccumulateGrad adds the chunk-B gradient into param.grad, which still views the wire tile
+                comp.append(("acq", [(("wire", r), "w", None)]))
+                comp.append(("rel", [(("wire", r), "w", None)]))
+            for c, (ev, grad, wire, par, carry) in enumerate((("mid", "gradA", "wireA", "paramsA", "carryA"),
+                                                              ("bwd", "gradB", "wire", "paramsB", "carryB"))):
+                comm.append(("wev", (ev, r, e)))
+                comm.append(("acq", [((grad, r, e), "r", e), ((carry, r), "w", 2 * e - 1), ((wire, r), "w", None)]))
+                comm.append(("rel", [((grad, r, e), "r", None), ((carry, r), "w", 2 * e), ((wire, r), "w", e)]))
+                if r != 0:
+                    comm.append(("sig", ("GRAD_READY", 0, r), prog(e, c)))
+                    continue
+                for p in range(1, n):
+                    comm.append(("wait", ("GRAD_READY", 0, p), prog(e, c)))
+                reads = [((wire, p), "r", e) for p in range(n)]
+                comm.append(("acq", reads + [((par, p), "w", None) for p in range(n)]))
+                comm.append(("rel", [(k, md, None) for k, md, _ in reads] + [((par, p), "w", e) for p in range(n)]))
+            if r == 0:
+                for p in range(n):
+                    comm.append(("sig", ("PARAMS_READY", p), e))
+            comm.append(("rec", ("done", r, e)))
+        m.add(f"r{r}.compute", comp)
+        m.add(f"r{r}.comm", comm)
+    _chunk_final(m, n, epochs)
+    return m
+
+
 def build_ps_unpipelined(n: int, epochs: int, drop: Optional[str] = None) -> Model:
     """``mode='ps'``, ``pipeline=False``: rank 0 gathers, updates and publishes in ONE launch inside ``step()``.
 
@@ -833,7 +888,7 @@ def build_stem_wgrad_pipeline(n: int = 1, epochs: int = 4, drop: Optional[str] =
 
 MODES = {"ps": build_ps, "ps_unpipelined": build_ps_unpipelined, "allgather": build_allgather,
          "allgather_unpipelined": build_allgather_unpipelined, "async": build_async, "stem_pipeline": build_stem_pipeline,
-         "stem_wgrad_pipeline": build_stem_wgrad_pipeline}
+         "stem_wgrad_pipeline": build_stem_wgrad_pipeline, "ps_accumulate": build_ps_accumulate}
 
 
 def check(mode: str, n: int, epochs: int, max_states: int = 2_000_000, **kw) -> Result:

@@ -27,6 +27,7 @@ plumbing configuration).
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import os
 import pickle
@@ -42,7 +43,7 @@ import torch
 from . import codings as _codings
 from . import mpi_comms as comms
 from . import runtime
-from .utils.misc import _bytes_of, find_param  # noqa: F401  (reference helpers, ps.py:25-50)
+from .utils.misc import MicroBatchCounter, _bytes_of, find_param  # noqa: F401  (reference helpers, ps.py:25-50)
 
 __all__ = ["MPI_PS", "SGD", "Adam", "_bytes_of", "find_param"]
 
@@ -164,6 +165,11 @@ class MPI_PS(torch.optim.Optimizer):
         self.timings: List[Dict[str, float]] = []
         self.futures: List[Any] = []
         self.names: List[str] = []
+        # gradient accumulation (no_sync): host engine — fp32 sum per parameter name, and the gradient dtype it is sent in
+        self._no_sync = False
+        self._carry: Dict[str, Any] = {}
+        self._accumulated = False       # a gradient was summed inside no_sync() since the last step()
+        self._mb = MicroBatchCounter()
         self.pool = ThreadPoolExecutor(max_workers=int(os.environ.get("PSB200_ENCODE_THREADS", "8")))
         self._inline_encode_bytes = int(os.environ.get("PSB200_INLINE_ENCODE_BYTES", 1 << 20))
         self._finalizer = weakref.finalize(self, self.pool.shutdown, False)
@@ -245,7 +251,23 @@ class MPI_PS(torch.optim.Optimizer):
         return msg, data
 
     def async_code(self, grad, *args, name=None, **kwargs):
-        """Backward hook: queue the encode on the pool and remember hook-firing order (``ps.py:98-101``)."""
+        """Backward hook: queue the encode on the pool and remember hook-firing order (``ps.py:98-101``).  Inside ``no_sync()``
+        the gradient is added to the name's fp32 carry instead; the next gradient of that name is sent as (carry + gradient),
+        rounded once to the gradient's dtype."""
+        self._mb.fire(name)
+        if self._no_sync:
+            self._accumulated = True
+            c = self._carry.get(name)
+            if c is None:
+                c = self._carry[name] = (torch.zeros(grad.shape, dtype=torch.float32, device=grad.device), grad.dtype)
+            c[0].add_(grad)
+            return
+        if name in self._carry:
+            c, _ = self._carry.pop(name)
+            grad = c.add_(grad).to(grad.dtype)
+        self._submit_encode(grad, *args, name=name, **kwargs)
+
+    def _submit_encode(self, grad, *args, name=None, **kwargs):
         if (not grad.is_cuda and grad.numel() * grad.element_size() <= self._inline_encode_bytes
                 and getattr(self.code, "cheap", False)):
             # small host gradient, trivial coding (identity / cast / scale): the pool hand-off (a GIL round trip per future,
@@ -263,6 +285,8 @@ class MPI_PS(torch.optim.Optimizer):
     # ------------------------------------------------------------------------------- step
     def step(self, closure=None):
         """Perform one optimization step; returns ``(loss, data)`` (``ps.py:103-193``)."""
+        if self._no_sync:
+            raise RuntimeError("step() inside no_sync(): leave the no_sync() block first (its gradients are summed, not sent)")
         loss = None
         if closure is not None:
             with torch.enable_grad():
@@ -270,16 +294,55 @@ class MPI_PS(torch.optim.Optimizer):
         self.steps += 1
         if self._engine is not None:
             data = self._engine.step()
-        elif self.mode == "allgather" or self.size == 1:
-            data = self._step_allgather()
-        elif self.mode == "ps":
-            data = self._step_ps()
         else:
-            data = self._step_async()
+            for name in list(self._carry):     # accumulated only inside no_sync(): the carry alone is this step's gradient
+                c, dtype = self._carry.pop(name)
+                self._submit_encode(c.to(dtype), name=name, encode=self.code.encode)
+            if self.mode == "allgather" or self.size == 1:
+                data = self._step_allgather()
+            elif self.mode == "ps":
+                data = self._step_ps()
+            else:
+                data = self._step_async()
+            data["micro_batches"] = self._mb.n
+            self._mb.reset()
+            self._accumulated = False
         self.timings.append(data)
         if len(self.timings) > 1024:
             del self.timings[:512]
         return loss, data
+
+    @contextlib.contextmanager
+    def no_sync(self):
+        """Gradient accumulation, like DDP's ``no_sync()``: backwards inside the block are summed locally and nothing is sent;
+        the next ``step()`` sends the sum over every backward since the last step, in one exchange::
+
+            opt.zero_grad(set_to_none=True)
+            for i, (x, y) in enumerate(micro_batches):
+                with opt.no_sync() if i < len(micro_batches) - 1 else contextlib.nullcontext():
+                    loss_fn(model(x), y).backward()
+            loss, data = opt.step()          # data["micro_batches"] == len(micro_batches)
+
+        The gradient sent is the plain sum: scale the loss for a mean (``average=True`` still divides by the number of ranks
+        only).  The sum is kept in fp32 and rounded to the wire once (DESIGN.md, wire numerics rule 12).  Running every backward
+        inside ``no_sync()`` and then calling ``step()`` gives the same bits; but then the whole exchange runs inside ``step()``,
+        whereas a last backward outside the block keeps the device engine's per-chunk pipeline under backward.  A parameter
+        that got a gradient in any backward of the step counts as having one.  ``step()`` and ``state_dict()`` raise while
+        gradients are accumulated and not sent.  On the dedicated server of ``mode='async'`` this is a no-op."""
+        if self._no_sync:
+            yield
+            return
+        if self._engine is not None:
+            self._engine.begin_no_sync()
+        self._no_sync = True
+        self._mb.cut()
+        try:
+            yield
+        finally:
+            self._no_sync = False
+            self._mb.cut()
+            if self._engine is not None:
+                self._engine.end_no_sync()
 
     # -- shared host-engine pieces ---------------------------------------------------------
     def _hyper(self, group) -> Dict[str, Any]:
@@ -583,6 +646,9 @@ class MPI_PS(torch.optim.Optimizer):
 
     # --------------------------------------------------------------------- checkpointing
     def state_dict(self):
+        if self._no_sync or self._accumulated or (self._engine is not None and self._engine.accumulating):
+            raise RuntimeError("state_dict() during gradient accumulation: the summed gradients are not checkpointed; "
+                               "call step() first")
         if self._engine is not None:
             self._engine.sync_state_to_torch()
         return super().state_dict()

@@ -116,3 +116,26 @@ def dump_chrome_trace(timings: Iterable[Dict[str, float]], path: str, pid: int =
                 t += dur
     with open(path, "w") as f:
         json.dump({"traceEvents": events, "displayTimeUnit": "ms"}, f)
+
+
+class MicroBatchCounter:
+    """Counts the backward passes summed into one step from hook firings: a new one starts at the first hook after ``reset()`` or
+    ``cut()`` (entering or leaving ``no_sync()``), or when a parameter fires again."""
+
+    def __init__(self):
+        self.reset()
+
+    def reset(self):
+        self.n, self._seen = 0, None
+
+    def cut(self):
+        self._seen = None
+
+    def fire(self, key) -> bool:
+        """Record a hook firing; True when it opens a new backward pass."""
+        if self._seen is not None and key not in self._seen:
+            self._seen.add(key)
+            return False
+        self.n += 1
+        self._seen = {key}
+        return True

@@ -21,7 +21,7 @@ OUT = os.path.join(ROOT, "profiles", "sm90a")
 KERNELS = [
     ("ps_kernels.o", r"psb_update_kernel<0, 1, 0>", "psb_update_kernel_dense_bf16_sgd"),
     ("ps_kernels.o", r"psb_update_kernel<2, 1, 1>", "psb_update_kernel_topk_bf16_adam"),
-    ("ps_kernels.o", r"psb_encode_kernel<2, 1>", "psb_encode_kernel_topk_bf16"),
+    ("ps_kernels.o", r"psb_encode_kernel<2, 1, false>", "psb_encode_kernel_topk_bf16"),
     ("ps_kernels.o", r"psb_select_kernel", "psb_select_kernel"),
     ("ps_kernels.o", r"psb_snapshot_fetch", "psb_snapshot_fetch"),
     ("bcast_gemm.o", r"psb_bcast_gemm_kernel<128, 2, 3>", "psb_bcast_gemm_kernel_pair_tma_store"),
