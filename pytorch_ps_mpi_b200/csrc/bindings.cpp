@@ -68,7 +68,7 @@ struct UpdatePlan {
   void launch(uint64_t epoch, const std::vector<std::vector<double>>& groups, uint32_t contrib_mask, double inv_count,
               int wait_grads, int signal_mode, uint32_t ack_mask, uint64_t version, uint64_t select_out,
               int average_dynamic, uint64_t active_ptr, double timeout_s, uint32_t wait_mask, uint64_t stream,
-              int tile_begin, int tile_end, uint64_t wait_value, uint64_t param_hyper) {
+              int tile_begin, int tile_end, uint64_t wait_value, uint64_t param_hyper, int state_shift) {
     if (groups.size() > PSB_MAX_GROUPS) throw std::runtime_error("too many param groups for one launch");
     for (size_t i = 0; i < groups.size(); ++i) {
       const auto& g = groups[i];
@@ -83,6 +83,9 @@ struct UpdatePlan {
     a.tile_begin = tile_end < 0 ? 0 : tile_begin;
     a.tile_end = tile_end < 0 ? a.ntiles : tile_end;
     if (a.tile_begin < 0 || a.tile_end > a.ntiles || a.tile_begin >= a.tile_end) throw std::runtime_error("bad tile range");
+    // compact optimizer state (mode='sharded'): tile t's state lives at (t - state_shift) * TILE; every window keeps it
+    if (state_shift < 0 || state_shift > a.tile_begin) throw std::runtime_error("bad state_shift");
+    a.state_shift = state_shift;
     a.wait_value = tile_end < 0 ? epoch : wait_value;
     a.contrib_mask = contrib_mask;
     a.wait_mask = wait_mask;
@@ -202,12 +205,17 @@ void accumulate(const std::vector<at::Tensor>& grads, const std::vector<int>& fi
 }
 
 void signal(const std::vector<uint64_t>& targets, int slot, uint64_t value, int extra_slot, uint64_t extra_value,
-            uint64_t stream, uint64_t version_local, int version_slot) {
+            uint64_t stream, uint64_t version_local, int version_slot, bool add) {
   std::vector<uint64_t*> t;
   for (auto p : targets) t.push_back(reinterpret_cast<uint64_t*>(p));
-  psb_launch_signal(pick_stream(stream), t.data(), (int)t.size(), slot, value,
-                    extra_slot >= 0 ? reinterpret_cast<uint64_t*>(1) : nullptr, extra_slot < 0 ? 0 : extra_slot, extra_value,
-                    reinterpret_cast<uint64_t*>(version_local), version_slot);
+  if (add) {
+    if (extra_slot >= 0 || version_local != 0) throw std::runtime_error("signal: add takes no extra / version slot");
+    psb_launch_signal_add(pick_stream(stream), t.data(), (int)t.size(), slot, value);
+  } else {
+    psb_launch_signal(pick_stream(stream), t.data(), (int)t.size(), slot, value,
+                      extra_slot >= 0 ? reinterpret_cast<uint64_t*>(1) : nullptr, extra_slot < 0 ? 0 : extra_slot, extra_value,
+                      reinterpret_cast<uint64_t*>(version_local), version_slot);
+  }
   check_launch("psb_signal_kernel launch");
 }
 
@@ -266,6 +274,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("SIGNAL_NONE") = (int)SIGNAL_NONE;
   m.attr("SIGNAL_PARAMS_READY") = (int)SIGNAL_PARAMS_READY;
   m.attr("SIGNAL_CONSUMED") = (int)SIGNAL_CONSUMED;
+  m.attr("SIGNAL_PARAMS_READY_ADD") = (int)SIGNAL_PARAMS_READY_ADD;
 
   py::class_<psb::SymmBlock, std::shared_ptr<psb::SymmBlock>>(m, "SymmBlock")
       .def(py::init<int, int, int, size_t, const std::string&>(), py::arg("rank"), py::arg("world"), py::arg("device"),
@@ -322,7 +331,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("inv_count"), py::arg("wait_grads"), py::arg("signal_mode"), py::arg("ack_mask") = 0,
            py::arg("version") = 0, py::arg("select_out") = 0, py::arg("average_dynamic") = 0, py::arg("active_ptr") = 0,
            py::arg("timeout_s") = 30.0, py::arg("wait_mask") = 0xffffffffu, py::arg("stream") = 0,
-           py::arg("tile_begin") = 0, py::arg("tile_end") = -1, py::arg("wait_value") = 0, py::arg("param_hyper") = 0);
+           py::arg("tile_begin") = 0, py::arg("tile_end") = -1, py::arg("wait_value") = 0, py::arg("param_hyper") = 0,
+           py::arg("state_shift") = 0);
 
   m.def("update_max_grid", &psb_update_max_grid);
   m.def("launch_count", []() { return (uint64_t)psb_launch_count(); }, "kernels of ours launched by this process so far");
@@ -336,7 +346,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("tiles_ptr"), py::arg("carry_ptr"), py::arg("stream") = 0,
         "gradient accumulation: carry (fp32, arena-shaped) += each gradient, one launch per PSB_ENCODE_MAX gradients");
   m.def("signal", &signal, py::arg("targets"), py::arg("slot"), py::arg("value"), py::arg("extra_slot") = -1,
-        py::arg("extra_value") = 0, py::arg("stream") = 0, py::arg("version_local") = 0, py::arg("version_slot") = 0);
+        py::arg("extra_value") = 0, py::arg("stream") = 0, py::arg("version_local") = 0, py::arg("version_slot") = 0,
+        py::arg("add") = false);
   m.def("wait_flags", &wait_flags, py::arg("signal_local"), py::arg("slot0"), py::arg("mask"), py::arg("want"),
         py::arg("timeout_s"), py::arg("stream") = 0);
   m.def("select_ready", &select_ready, py::arg("signal_local"), py::arg("consumed"), py::arg("cand_mask"), py::arg("quota"),

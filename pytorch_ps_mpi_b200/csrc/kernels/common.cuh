@@ -33,7 +33,8 @@ enum : int { BCAST_LOCAL = 0, BCAST_UNICAST = 1, BCAST_MULTICAST = 2 };
 // how the gradient tiles are gathered
 enum : int { REDUCE_P2P = 0, REDUCE_NVLS = 1 };
 // which flag the last CTA of an update launch raises on every rank
-enum : int { SIGNAL_NONE = 0, SIGNAL_PARAMS_READY = 1, SIGNAL_CONSUMED = 2 };
+// (SIGNAL_PARAMS_READY_ADD: mode='sharded' — every server adds 1 to every rank's PARAMS_READY, so the slot counts servers done)
+enum : int { SIGNAL_NONE = 0, SIGNAL_PARAMS_READY = 1, SIGNAL_CONSUMED = 2, SIGNAL_PARAMS_READY_ADD = 3 };
 
 // signal-pad slots (uint64 each); pad is PSB_SIGNAL_SLOTS * 8 bytes at the start of the block
 #define PSB_SIGNAL_SLOTS 512
@@ -316,6 +317,14 @@ PSB_HD inline uint32_t ld_sys_u32(const void* p) {
   return v;
 #else
   return *static_cast<const uint32_t*>(p);
+#endif
+}
+// System-scope release add (a counting flag: PARAMS_READY in mode='sharded'); on the host an atomic add with release order.
+PSB_HD inline void red_release_sys_add_u64(uint64_t* p, uint64_t v) {
+#ifdef __CUDA_ARCH__
+  asm volatile("red.release.sys.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+#else
+  __atomic_fetch_add(p, v, __ATOMIC_RELEASE);
 #endif
 }
 

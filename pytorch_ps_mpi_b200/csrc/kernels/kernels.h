@@ -75,7 +75,11 @@ struct UpdateArgs {
   int32_t tile_begin, tile_end;        // this launch covers arena tiles [tile_begin, tile_end) — one chunk of the
                                        // pipeline (or the whole arena)
   int32_t wait_grads;                  // spin on SIG_GRAD_READY of every contributor first
-  int32_t signal_mode;                 // SIGNAL_NONE | SIGNAL_PARAMS_READY → all | SIGNAL_CONSUMED[rank] → all
+  int32_t signal_mode;                 // SIGNAL_NONE | SIGNAL_PARAMS_READY → all | SIGNAL_CONSUMED[rank] → all |
+                                       // SIGNAL_PARAMS_READY_ADD (+1 on every rank's PARAMS_READY)
+  int32_t state_shift;                 // master / buf0-2 hold tile t at (t - state_shift) * PSB_TILE: a server's compact state
+                                       // for the tiles it serves (mode='sharded'); 0 = arena-indexed.  Publication and
+                                       // param_local keep the arena index.
   uint32_t ack_mask;                   // async: ranks to acknowledge (SIG_ACK) when done
   int32_t ack_last;                    // 1 on the last window of a launch sequence: the async contributors (chosen on the
                                        // device, select_out) are acknowledged only then
@@ -94,6 +98,8 @@ void psb_launch_update(cudaStream_t s, int kind, int wire, int opt, const Update
 void psb_launch_signal(cudaStream_t s, uint64_t* const* targets, int ntargets, int slot, uint64_t value,
                        uint64_t* extra_slot_base, int extra_slot, uint64_t extra_value, uint64_t* version_local = nullptr,
                        int version_slot = 0);
+// targets[t][slot] += value (release add; mode='sharded': a server's PARAMS_READY count when its last launch updated nothing)
+void psb_launch_signal_add(cudaStream_t s, uint64_t* const* targets, int ntargets, int slot, uint64_t value);
 void psb_launch_wait(cudaStream_t s, const uint64_t* signal_local, int slot0, uint32_t mask, uint64_t want,
                      unsigned long long timeout_ns);
 // async PS: block until >= quota workers of `cand_mask` have SIG_GRAD_READY > consumed[r]; writes the

@@ -775,6 +775,12 @@ __global__ void __launch_bounds__(PSB_THREADS, 3) psb_update_kernel(const __grid
         st_release_sys(a.signal_peer[tid] + SIG_PARAMS_READY, a.epoch);
       } else if (a.signal_mode == SIGNAL_CONSUMED) {
         st_release_sys(a.signal_peer[tid] + SIG_CONSUMED + a.rank, a.epoch);
+      } else if (a.signal_mode == SIGNAL_PARAMS_READY_ADD) {
+        // mode='sharded': N servers each add 1 after publishing their share, so e*N means "all of step e is published".
+        // Adds are read-modify-writes of one location, so they form a release sequence (PTX memory model): an acquire
+        // that reads e*N — the value written by the LAST add — synchronizes with EVERY earlier release-add, and thus sees
+        // every server's parameter stores, not only the last server's.
+        red_release_sys_add_u64(a.signal_peer[tid] + SIG_PARAMS_READY, 1ull);
       }
       if (ack >> tid & 1u) {
         const uint64_t e = ld_relaxed_sys_u64(a.signal_local + SIG_GRAD_READY + tid);
@@ -799,6 +805,7 @@ struct SignalArgs {
   // pass that produced this one started) into targets[t][version_slot], then re-samples the latest published version.
   uint64_t* version_local;
   int32_t version_slot;
+  int32_t add;       // targets[t][slot] += value instead of the store (a server of mode='sharded' that updated nothing last)
 };
 
 __global__ void psb_signal_kernel(const __grid_constant__ SignalArgs a) {
@@ -809,7 +816,10 @@ __global__ void psb_signal_kernel(const __grid_constant__ SignalArgs a) {
   if (t < a.n) {
     if (a.extra_base != nullptr && a.targets[t] != nullptr) st_release_sys(a.targets[t] + a.extra_slot, a.extra_value);
     if (a.version_local != nullptr && a.targets[t] != nullptr) st_release_sys(a.targets[t] + a.version_slot, seen);
-    if (a.targets[t] != nullptr) st_release_sys(a.targets[t] + a.slot, a.value);
+    if (a.targets[t] != nullptr) {
+      if (a.add) red_release_sys_add_u64(a.targets[t] + a.slot, a.value);
+      else st_release_sys(a.targets[t] + a.slot, a.value);
+    }
   }
   __syncwarp();      // every lane has read `seen` before lane 0 replaces it (several targets: one lane each)
   if (a.version_local != nullptr && t == 0)
@@ -970,7 +980,21 @@ template <int KIND, int WIRE, int OPT>
 void launch_update_t(cudaStream_t s, const UpdateArgs& a, int grid) {
   // (a variant with two P2P tiles in flight per thread and no state prefetch measured slower on the ResNet-18 arena at
   //  N = 1, and was removed)
-  psb_update_kernel<KIND, WIRE, OPT><<<grid, PSB_THREADS, 0, s>>>(a);
+  if (a.state_shift == 0) {
+    psb_update_kernel<KIND, WIRE, OPT><<<grid, PSB_THREADS, 0, s>>>(a);
+    return;
+  }
+  // compact optimizer state (mode='sharded'): the kernel indexes master / buf0-2 by arena element, so hand it those pointers
+  // moved back by state_shift tiles — it only ever touches elements of tiles >= state_shift, i.e. the compact buffers.  A
+  // shift applied to the pointers here costs the kernel nothing: an index shift inside it cost registers and spills.
+  UpdateArgs b = a;
+  const size_t d = (size_t)a.state_shift * PSB_TILE;
+  if (b.master) b.master -= d;
+  if (b.buf0) b.buf0 -= d;
+  if (b.buf1) b.buf1 -= d;
+  if (b.buf2) b.buf2 -= d;
+  b.state_shift = 0;
+  psb_update_kernel<KIND, WIRE, OPT><<<grid, PSB_THREADS, 0, s>>>(b);
 }
 template <int KIND, int WIRE>
 void launch_update_o(cudaStream_t s, int opt, const UpdateArgs& a, int grid) {
@@ -1062,6 +1086,17 @@ void psb_launch_signal(cudaStream_t s, uint64_t* const* targets, int ntargets, i
   a.extra_value = extra_value;
   a.version_local = version_local;
   a.version_slot = version_slot;
+  psb_signal_kernel<<<1, 32, 0, s>>>(a);
+  psb_count_launch(1);
+}
+
+void psb_launch_signal_add(cudaStream_t s, uint64_t* const* targets, int ntargets, int slot, uint64_t value) {
+  SignalArgs a{};
+  a.n = ntargets;
+  for (int i = 0; i < ntargets && i < PSB_MAX_RANKS; ++i) a.targets[i] = targets[i];
+  a.slot = slot;
+  a.value = value;
+  a.add = 1;
   psb_signal_kernel<<<1, 32, 0, s>>>(a);
   psb_count_launch(1);
 }

@@ -9,9 +9,9 @@ nothing goes through NCCL/MPI):
    block-wise top-k), overlapping with the rest of backward;
 2. ``step()`` raises this rank's ``GRAD_READY`` epoch flag (``st.release.sys`` into the server's
    signal pad — the ``Igatherv`` post of ``mpi_comms.py:88``);
-3. the server (rank 0 in ``mode='ps'``; every rank in ``mode='allgather'``) launches
-   ``psb_update_kernel`` once: wait flags → pull every rank's wire tiles over NVLink (or one
-   ``multimem.ld_reduce`` through the switch) → decode + rank-ordered fp32 sum → SGD/Adam on fp32
+3. the server (rank 0 in ``mode='ps'``; every rank in ``mode='allgather'``; in ``mode='sharded'`` every rank for its own
+   share of each chunk, see ``_make_shards``) launches ``psb_update_kernel`` once: wait flags → pull every rank's wire
+   tiles over NVLink (or one ``multimem.ld_reduce`` through the switch) → decode + rank-ordered fp32 sum → SGD/Adam on fp32
    master state → publish the new parameter tiles into every rank's *symmetric parameter
    arena* (``multimem.st`` or peer stores) → raise ``PARAMS_READY``;
 4. workers queue a one-thread wait kernel on their compute stream (the ``req.Wait()`` of
@@ -64,6 +64,8 @@ class DeviceEngine:
         if len(opt.param_groups) > self.m.MAX_GROUPS:
             raise ValueError(f"device engine supports up to {self.m.MAX_GROUPS} param groups")
         self.mode = opt.mode
+        # mode='sharded': every rank serves one contiguous share of every chunk (N = 1 is mode='ps')
+        self.sharded = self.mode == "sharded" and opt.size > 1
         names = {id(p): n for n, p in opt._named.items()}
         self.layout = FlatLayout(opt.param_groups, names)
         p0 = self.layout.slots[0].param
@@ -81,7 +83,7 @@ class DeviceEngine:
         self.timeout_s = float(os.environ.get("PSB200_DEVICE_TIMEOUT", "900"))
         self.chunk_bytes = int(os.environ.get("PSB200_CHUNK_BYTES", os.environ.get("PSB200_BUCKET_BYTES", 4 << 20)))
         self.pipeline = bool(getattr(opt, "pipeline", True)) and os.environ.get("PSB200_PIPELINE", "1") != "0" \
-            and self.mode in ("ps", "allgather")
+            and self.mode in ("ps", "allgather", "sharded")
         L = self.layout
         nt, n_pad = L.ntiles, L.numel_padded
         self._check_same_layout_everywhere()
@@ -129,8 +131,12 @@ class DeviceEngine:
             torch.cuda.synchronize(self.device)
             self.world.barrier()
 
-        # ---- server-side state ----
-        self.is_server = (self.mode == "allgather") or self.rank == 0 or self.size == 1
+        # ---- the pipeline chunks: contiguous runs of whole parameters in arena (= backward) order ----
+        self._make_chunks()
+        self._make_shards()
+
+        # ---- server-side state (mode='sharded': compact, only the tiles this rank serves) ----
+        self.is_server = self.mode in ("allgather", "sharded") or self.rank == 0 or self.size == 1
         self.tiles = L.tile_table_fast().to(self.device)
         self.amax = torch.zeros(max(L.nparams, 1), dtype=torch.int32, device=self.device)
         self.active_dev = torch.ones(max(L.nparams, 1), dtype=torch.uint8, device=self.device)
@@ -151,16 +157,19 @@ class DeviceEngine:
         self._mb = MicroBatchCounter()
         self.master = self.buf0 = self.buf1 = self.buf2 = None
         if self.is_server:
+            n_state = self.state_tiles * TILE if self.sharded else n_pad
             if self.dtype != torch.float32 and master_fp32:
-                self.master = self.param_arena.float()
+                self.master = torch.empty(n_state, dtype=torch.float32, device=self.device)
+                self._to_state(self.param_arena, self.master)
             need_b0 = opt.optim == "adam" or any(g.get("momentum", 0) != 0 for g in opt.param_groups)
             if need_b0:
-                self.buf0 = torch.zeros(n_pad, dtype=torch.float32, device=self.device)
+                self.buf0 = torch.zeros(n_state, dtype=torch.float32, device=self.device)
             if opt.optim == "adam":
-                self.buf1 = torch.zeros(n_pad, dtype=torch.float32, device=self.device)
+                self.buf1 = torch.zeros(n_state, dtype=torch.float32, device=self.device)
                 if any(g.get("amsgrad", False) for g in opt.param_groups):
-                    self.buf2 = torch.zeros(n_pad, dtype=torch.float32, device=self.device)
-            self._expose_state()
+                    self.buf2 = torch.zeros(n_state, dtype=torch.float32, device=self.device)
+            if not self.sharded:
+                self._expose_state()
         self._group_steps = [0] * len(opt.param_groups)
         self._hyper_cache = None
         # per-parameter step counts (the reference keeps optimizer state per parameter and skips p.grad is None,
@@ -191,7 +200,7 @@ class DeviceEngine:
         # fp32 and returns the sum rounded once to the wire type (|rel err| <= 2^-9 for bf16) before the fp32 master
         # update.  allgather keeps the rank-ordered P2P sum (every rank must produce bit-identical sums), async keeps
         # it because only the selected contributors may be summed.  'nvls' / 'p2p' force either.
-        auto_nvls = (nvls_ok and self.mode == "ps" and self.size >= 4
+        auto_nvls = (nvls_ok and self.mode in ("ps", "sharded") and self.size >= 4
                      and os.environ.get("PSB200_REDUCE", "") != "p2p")
         if reduce == "p2p":
             self.reduce = REDUCE_P2P
@@ -236,8 +245,6 @@ class DeviceEngine:
         # run draws.
         self._qsgd_step = 0
         self._sig_base = [p + self.off_signal for p in self.arena.ptrs]
-        # ---- the pipeline chunks: contiguous runs of whole parameters in arena (= backward) order ----
-        self._make_chunks()
         self._start_step()
         self._keep_prev: List[torch.Tensor] = []   # last step's gradients: freed one step late (see _flush)
         self._prev_done = None                      # comm-stream completion of the last step
@@ -262,7 +269,7 @@ class DeviceEngine:
         self._async_last = {"contributors": [], "param_version": 0, "staleness": {}, "updates_applied": 0}
         # K10 "no separate serialization pass": producers we own (our BN / stem / linear backward kernels) write their
         # gradient straight into this rank's wire arena when the wire layout IS the gradient layout
-        self._direct_ok = (self.kind == KIND_DENSE and self.wire == wire_code_of(self.dtype) and self.mode == "ps"
+        self._direct_ok = (self.kind == KIND_DENSE and self.wire == wire_code_of(self.dtype) and self.mode in ("ps", "sharded")
                            and os.environ.get("PSB200_DIRECT_GRAD", "1") != "0")
         self.direct_grads = 0
         self.direct_names: set = set()
@@ -320,6 +327,49 @@ class DeviceEngine:
             for sl in c:
                 self._chunk_of[sl.index] = k
 
+    def _make_shards(self):
+        """``mode='sharded'``: static split of every chunk ``[lo, hi)`` into ``N`` contiguous tile ranges, one per rank in rank
+        order (identical on every rank: it depends on the layout only).  Each rank gets ``(hi - lo) // N`` tiles; the remainder
+        goes one tile each to the ``(hi - lo) % N`` ranks starting at ``k % N``, so small chunks do not all land on rank 0.
+
+        A rank keeps optimizer state only for its own ranges, concatenated in chunk order (``state_tiles`` tiles): the update of
+        chunk ``k`` addresses it with ``state_shift = lo_mine - compact_base``.  Tile granularity is exact for every coding: they
+        all decode per tile and read per-parameter scales and hyper-parameters by index."""
+        n = self.size
+        self.shards = []                      # per chunk: [(begin, end)] per rank
+        self._mine = []                       # per chunk: (begin, end, state_shift) of this rank
+        base = 0
+        spans = self.chunk_tiles if self.pipeline else [(0, self.layout.ntiles)]
+        for k, (lo, hi) in enumerate(spans):
+            q, rem = divmod(hi - lo, n)
+            ranges, b = [], lo
+            for r in range(n):
+                e = b + q + (1 if (r - k) % n < rem else 0)
+                ranges.append((b, e))
+                b = e
+            self.shards.append(ranges)
+            mb, me = ranges[self.rank]
+            self._mine.append((mb, me, mb - base))
+            base += me - mb
+        self.state_tiles = base
+
+    def _state_pieces(self, first_tile: int, ntiles: int):
+        """``(arena_tile_lo, arena_tile_hi, state_tile_lo)`` for the parts of arena tiles ``[first_tile, first_tile + ntiles)``
+        whose optimizer state this rank keeps: all of them (one piece, state index = arena index) unless ``mode='sharded'``."""
+        if not self.sharded:
+            return [(first_tile, first_tile + ntiles, first_tile)]
+        out = []
+        for b, e, shift in self._mine:
+            lo, hi = max(b, first_tile), min(e, first_tile + ntiles)
+            if lo < hi:
+                out.append((lo, hi, lo - shift))
+        return out
+
+    def _to_state(self, full: torch.Tensor, state: torch.Tensor):
+        """Copy the arena-indexed ``full`` into ``state`` (compact in mode='sharded')."""
+        for lo, hi, c in self._state_pieces(0, self.layout.ntiles):
+            state[c * TILE: (c + hi - lo) * TILE].copy_(full[lo * TILE: hi * TILE])
+
     def _start_step(self):
         """The bookkeeping of a step no gradient has arrived for yet.  Callers decide what happens to the gradients kept
         alive for the previous step (``_keep_prev``) and to its completion event (``_prev_done``)."""
@@ -369,6 +419,55 @@ class DeviceEngine:
             return
         for s in self.layout.slots:   # SGD too: the first-step momentum rule (ps.py:203-205) needs it on resume
             o.state[s.param]["step"] = self._param_steps[s.index] if self.mode != "async" else self._group_steps[s.group]
+        if self.sharded:
+            self._gather_state()
+
+    def _state_buffers(self):
+        """``(state key, flat fp32 buffer)`` of every optimizer-state buffer this engine keeps."""
+        o = self.opt
+        out = (("momentum_buffer", self.buf0 if o.optim == "sgd" else None), ("exp_avg", self.buf0 if o.optim == "adam" else None),
+               ("exp_avg_sq", self.buf1), ("max_exp_avg_sq", self.buf2), ("master_param", self.master))
+        return [(k, b) for k, b in out if b is not None]
+
+    def _gather_state(self):
+        """mode='sharded' ``state_dict()`` (collective): every rank's compact shards → the full per-parameter state on every
+        rank, the values rank 0 holds in mode='ps', as CPU copies.  ``MPI_PS.state_dict`` drops them from ``opt.state`` once
+        its dict is built (:meth:`drop_state_copies`), so only the returned dict keeps them."""
+        torch.cuda.current_stream(self.device).wait_stream(self.comm_stream)
+        torch.cuda.synchronize(self.device)
+        bufs = self._state_buffers()
+        every = self.world.all_gather_object({k: b.cpu() for k, b in bufs})
+        full = {k: torch.zeros(self.layout.numel_padded, dtype=torch.float32) for k, _ in bufs}
+        for r, theirs in enumerate(every):
+            base = 0
+            for ranges in self.shards:
+                b, e = ranges[r]
+                for k in full:
+                    full[k][b * TILE: e * TILE] = theirs[k][base * TILE: (base + e - b) * TILE]
+                base += e - b
+        o = self.opt
+        for s in self.layout.slots:
+            for k, flat in full.items():
+                o.state[s.param][k] = s.view(flat[s.offset: s.offset + s.numel])
+
+    def drop_state_copies(self):
+        """mode='sharded': leave only the step counts in ``opt.state`` — the engine's compact buffers are the live state, and
+        full-size copies (gathered for ``state_dict()``, or put there by ``load_state_dict()``) would undo the 1/N."""
+        o = self.opt
+        for s in self.layout.slots:
+            if s.param in o.state:      # a new dict: one that state_dict() already returned keeps its tensors
+                o.state[s.param] = {k: v for k, v in o.state[s.param].items()
+                                    if k in ("step", "qsgd_step") or not torch.is_tensor(v)}
+
+    def _load_slot(self, s, buf: torch.Tensor, value: torch.Tensor):
+        """Write parameter-shaped ``value`` into the state buffer ``buf`` at slot ``s`` (only this rank's tiles when sharded)."""
+        if not self.sharded:
+            s.view(buf[s.offset: s.offset + s.numel]).copy_(value.to(buf.dtype))
+            return
+        tmp = torch.zeros(s.ntiles * TILE, dtype=buf.dtype, device=buf.device)
+        s.view(tmp[: s.numel]).copy_(value.to(buf.dtype))
+        for lo, hi, c in self._state_pieces(s.first_tile, s.ntiles):
+            buf[c * TILE: (c + hi - lo) * TILE].copy_(tmp[(lo - s.first_tile) * TILE: (hi - s.first_tile) * TILE])
 
     def sync_state_from_torch(self, original=None):
         """After ``load_state_dict``: copy loaded tensors back into the flat (fp32) state.
@@ -388,13 +487,10 @@ class DeviceEngine:
                 if original is not None and id(s.param) in original:
                     st = original[id(s.param)]
                 sl = slice(s.offset, s.offset + s.numel)
-                for key, buf in (("momentum_buffer", self.buf0 if o.optim == "sgd" else None),
-                                 ("exp_avg", self.buf0 if o.optim == "adam" else None),
-                                 ("exp_avg_sq", self.buf1), ("max_exp_avg_sq", self.buf2),
-                                 ("master_param", self.master)):
-                    if buf is not None and key in st and st[key] is not None:
-                        if st[key].data_ptr() != buf[sl].data_ptr():
-                            s.view(buf[sl]).copy_(st[key].to(buf.dtype))
+                for key, buf in self._state_buffers():
+                    if key in st and st[key] is not None:
+                        if self.sharded or st[key].data_ptr() != buf[sl].data_ptr():
+                            self._load_slot(s, buf, st[key])
                 if "step" in st:
                     self._group_steps[s.group] = max(self._group_steps[s.group], int(st["step"]))
                     self._param_steps[s.index] = int(st["step"])
@@ -403,10 +499,13 @@ class DeviceEngine:
                 for s in self.layout.slots:
                     src = original.get(id(s.param), {}) if original is not None else o.state.get(s.param, {})
                     if "master_param" not in src:
-                        s.view(self.master[s.offset: s.offset + s.numel]).copy_(s.param.data.float())
+                        self._load_slot(s, self.master, s.param.data)
         if any(self._param_steps[s.index] != self._group_steps[s.group] for s in self.layout.slots):
             self._uniform_steps = False
-        self._expose_state()
+        if self.sharded:
+            self.drop_state_copies()
+        else:
+            self._expose_state()
 
     # ------------------------------------------------------------------------------- backward
     def grad_out(self, param: torch.nn.Parameter) -> Optional[torch.Tensor]:
@@ -416,8 +515,9 @@ class DeviceEngine:
         With Identity / same-dtype wires the wire tile of a parameter is bit-for-bit its gradient, so a kernel we own
         (fused BN backward, the stem's implicit weight gradient, ``BcastLinear``'s dW GEMM with ``out=``) can skip the
         ``psb_encode_kernel`` copy: ``on_grad`` recognises the pointer and only counts the parameter as arrived.  Safe in
-        ``mode='ps'`` only: a worker's backward starts after it observed PARAMS_READY (the server finished reading the
-        previous wire tiles); in ``allgather`` mode peers may still be reading them (CONSUMED is awaited on the comm stream)."""
+        ``mode='ps'`` and ``mode='sharded'`` only: a rank's backward starts after it observed PARAMS_READY (every server
+        finished reading the previous wire tiles); in ``allgather`` mode peers may still be reading them (CONSUMED is awaited
+        on the comm stream)."""
         if not self._direct_ok or self._closed or self.accumulating:
             return None                      # (an accumulated step encodes from the carry)
         sl = self.layout.by_id.get(id(param))
@@ -603,7 +703,9 @@ class DeviceEngine:
         elif sig:                                     # nothing fired in this chunk: the flag alone
             m.signal(sig[0], sig[1], sig[2], -1, 0, csh)
             self.launches += 1
-        if sync and self.is_server and (self.pipeline or last):
+        if self.sharded and (self.pipeline or last):
+            self._serve_shard(k if self.pipeline else 0, epoch, last, active_ptr)
+        elif sync and self.is_server and (self.pipeline or last):
             lo, hi = self.chunk_tiles[k] if self.pipeline else (0, self.layout.ntiles)
             inv = (1.0 / n) if self.opt.average else 1.0
             prof = self._prof.enabled
@@ -629,6 +731,33 @@ class DeviceEngine:
             self.launches += 1
             if prof:
                 self._update_spans.append((ev_a, self._prof.mark(cs)))
+
+    def _serve_shard(self, k: int, epoch: int, last: bool, active_ptr: int):
+        """``mode='sharded'``: wait for every peer's chunk-``k`` progress, then gather / update / publish this rank's share of
+        chunk ``k`` (to every rank).  The step's last launch adds 1 to every rank's PARAMS_READY instead of storing the epoch,
+        so the slot reaches ``epoch * N`` once all N servers have published; a rank with no tile in the last chunk adds its 1
+        with the signal kernel, still behind a wait for the peers' last progress value."""
+        m, csh, n = self.m, self._cs, self.size
+        lo, hi, shift = self._mine[k]
+        if hi <= lo and not last:
+            return
+        wait_mask = ((1 << n) - 1) & ~(1 << self.rank)
+        want = self._progress(epoch, k if self.pipeline else self.nchunks - 1)
+        m.wait_flags(self.arena.local_ptr + self.off_signal, m.SIG_GRAD_READY, wait_mask, want, self.timeout_s, csh)
+        self.launches += 1
+        if hi <= lo:
+            m.signal(self._sig_base, m.SIG_PARAMS_READY, 1, stream=csh, add=True)
+            self.launches += 1
+            return
+        prof = self._prof.enabled
+        ev_a = self._prof.mark(self.comm_stream) if prof else None
+        self.plan.launch(epoch, self._get_hypers(), (1 << n) - 1, (1.0 / n) if self.opt.average else 1.0, 0,
+                         m.SIGNAL_PARAMS_READY_ADD if last else SIGNAL_NONE,
+                         active_ptr=active_ptr, timeout_s=self.timeout_s, wait_mask=wait_mask, stream=csh,
+                         tile_begin=lo, tile_end=hi, wait_value=want, param_hyper=self._phyper_ptr, state_shift=shift)
+        self.launches += 1
+        if prof:
+            self._update_spans.append((ev_a, self._prof.mark(self.comm_stream)))
 
     def _before_first_encode(self):
         """Queued on the comm stream before this step's first write into the wire arena."""
@@ -772,6 +901,11 @@ class DeviceEngine:
                 m.wait_flags(self._sig_base[self.rank], m.SIG_PARAMS_READY, 1, epoch, self.timeout_s)
                 self.launches += 1
             # else: the first forward GEMM (BcastLinear / the stem) acquires the flag inside its TMA producer
+        elif self.sharded:
+            # every rank, rank 0 included: the other shards arrive from peers, so `done` of this rank's comm stream is not enough
+            if not self._gates:
+                m.wait_flags(self._sig_base[self.rank], m.SIG_PARAMS_READY, 1, epoch * self.size, self.timeout_s)
+                self.launches += 1
         else:
             cur.wait_event(done)
         data["comm_wait"] = time.time() - t3
@@ -892,7 +1026,7 @@ class DeviceEngine:
         if self.master is not None:
             torch.cuda.current_stream(self.device).wait_stream(self.comm_stream)
             with torch.no_grad():
-                self.master.copy_(self.param_arena)
+                self._to_state(self.param_arena, self.master)
 
     # ------------------------------------------------------------------------------ async mode
     def _step_async(self, data):
@@ -1032,21 +1166,29 @@ class DeviceEngine:
 
     def gate(self):
         """``(flag_ptr, epoch)`` the next forward must observe before reading broadcast weights.  Taking it marks the
-        current epoch's broadcast as acquired by a gated kernel (see :meth:`ensure_params`)."""
-        if self.size == 1 or self.mode != "ps" or self.rank == 0 or self._epoch == 0:
+        current epoch's broadcast as acquired by a gated kernel (see :meth:`ensure_params`).  In ``mode='sharded'`` the flag
+        counts servers: the value is ``epoch * N``, on every rank."""
+        if not self._gated():
             return 0, 0
         self._gate_epoch = self._epoch
-        return self.arena.local_ptr + self.off_signal + 8 * self.m.SIG_PARAMS_READY, self._epoch
+        return self.arena.local_ptr + self.off_signal + 8 * self.m.SIG_PARAMS_READY, self._params_ready_value()
+
+    def _gated(self) -> bool:
+        """Does the next forward have to acquire PARAMS_READY (a worker of mode='ps', every rank of mode='sharded')?"""
+        return self.size > 1 and self._epoch > 0 and (self.sharded or (self.mode == "ps" and self.rank != 0))
+
+    def _params_ready_value(self) -> int:
+        return self._epoch * self.size if self.sharded else self._epoch
 
     def ensure_params(self):
         """For forwards that bypass the gated kernel (eval mode, unsupported shapes) while a gate is registered: queue
         the plain wait kernel on the current stream unless this epoch's broadcast was already acquired."""
-        if self.size == 1 or self.mode != "ps" or self.rank == 0 or self._epoch == 0 or not self._gates:
+        if not self._gated() or not self._gates:
             return
         if self._gate_epoch == self._epoch:
             return
         self._gate_epoch = self._epoch
-        self.m.wait_flags(self._sig_base[self.rank], self.m.SIG_PARAMS_READY, 1, self._epoch, self.timeout_s)
+        self.m.wait_flags(self._sig_base[self.rank], self.m.SIG_PARAMS_READY, 1, self._params_ready_value(), self.timeout_s)
         self.launches += 1
 
     def peer_param_ptr(self, param: torch.Tensor, rank: int) -> int:

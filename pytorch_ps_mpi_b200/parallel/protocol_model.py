@@ -36,7 +36,7 @@ import sys
 from dataclasses import dataclass, field
 from typing import Dict, FrozenSet, Iterable, List, Optional, Sequence, Tuple
 
-__all__ = ["Violation", "Result", "Model", "build_ps", "build_ps_unpipelined", "build_allgather", "build_allgather_unpipelined", "build_async", "build_ps_accumulate", "build_stem_pipeline", "build_stem_wgrad_pipeline",
+__all__ = ["Violation", "Result", "Model", "build_ps", "build_ps_unpipelined", "build_allgather", "build_allgather_unpipelined", "build_async", "build_ps_accumulate", "build_sharded", "build_stem_pipeline", "build_stem_wgrad_pipeline",
            "check", "MODES"]
 
 DONE = 1 << 62          # device_engine._DONE_EPOCH / PSB_DONE_EPOCH
@@ -86,6 +86,7 @@ class Model:
 # Script ops (tuples):
 #   ("rec", ev) / ("wev", ev)                  CUDA event record / stream-wait-event
 #   ("sig", key, value)                        store `value` into flag slot `key`
+#   ("add", key, delta)                        flag slot `key` += delta (a release add: a counting flag)
 #   ("wait", key, value)                       spin until slot >= value
 #   ("acq", [(res, mode, expect), ...])        a kernel starts accessing resources ('r' / 'w'; expect = version or None)
 #   ("rel", [(res, mode, newver), ...])        the kernel finished (a write leaves version `newver`)
@@ -121,7 +122,7 @@ class _Explorer:
                 k = op[0]
                 if k in ("rec", "wev"):
                     model.flag(("ev", op[1]))
-                elif k in ("sig", "wait"):
+                elif k in ("sig", "add", "wait"):
                     model.flag(op[1])
                 elif k == "load":
                     self.observed.add(model.flag(op[2]))
@@ -159,7 +160,7 @@ class _Explorer:
             return st[1][self.m.flag(("ev", op[1]))] >= 1
         if k == "wait":
             return st[1][self.m.flag(op[1])] >= op[2]
-        if k == "sig":
+        if k in ("sig", "add"):
             return self.m.flag(op[1]) not in self.observed
         if k in ("jne", "jeqc", "mov"):
             return True
@@ -252,6 +253,8 @@ class _Explorer:
             pass
         elif k == "sig":
             flags = _set(flags, m.flag(op[1]), op[2])
+        elif k == "add":
+            flags = _set(flags, m.flag(op[1]), flags[m.flag(op[1])] + op[2])
         elif k == "acq":
             locs2 = _set(locs, i, (pc, regs, False, -1))
             st2 = self.acquire((locs2, flags, vers, infl), i, op[1], trace)
@@ -609,6 +612,64 @@ def build_ps_accumulate(n: int, epochs: int, drop: Optional[str] = None) -> Mode
     return m
 
 
+def build_sharded(n: int, epochs: int, drop: Optional[str] = None) -> Model:
+    """``mode='sharded'`` (pipelined, two chunks A and B): rank ``s`` serves shard ``s`` of each chunk.  Every rank encodes
+    its whole gradient and raises its GRAD_READY progress in every peer's pad; the owner of a shard waits for every peer's
+    progress, reads shard ``s`` of every rank's wire chunk and writes parameter shard ``s`` on every rank.  After its chunk-B
+    shard each rank adds 1 to every rank's PARAMS_READY, and the next step's forward waits for ``>= e * N`` (every rank,
+    rank 0 included).  Parameter and wire resources are per shard.
+
+    ``drop``: ``'params_ready'`` (no wait before the forward), ``'count_short'`` (wait for ``e * (N - 1)`` only),
+    ``'grad_ready'`` (the owner of B's shard 0 skips one peer's wait), ``'signal_server_only'`` (GRAD_READY goes to rank 0
+    only, as in mode='ps') — each must be caught."""
+    m = Model()
+    prog = lambda e, c: (e - 1) * 2 + c + 1      # noqa: E731
+    for r in range(n):
+        comp, comm = [], []
+        peers = [p for p in range(n) if p != r]
+        for e in range(1, epochs + 1):
+            if e > 1 and drop != "params_ready":
+                comp.append(("wait", ("PARAMS_READY", r), (e - 1) * (n - 1 if drop == "count_short" else n)))
+            if e > 1:
+                comp.append(("wev", ("done", r, e - 1)))                   # _flush_chunk: at most one step ahead
+            pa = [(("paramsA", s, r), "r", e - 1) for s in range(n)]
+            pb = [(("paramsB", s, r), "r", e - 1) for s in range(n)]
+            comp.append(("acq", pa + pb + [(("gradA", r, e), "w", None)]))
+            comp.append(("rel", [(k, md, None) for k, md, _ in pa] + [(("gradA", r, e), "w", e)]))
+            comp.append(("rec", ("mid", r, e)))
+            comp.append(("acq", [(("gradB", r, e), "w", None)]))
+            comp.append(("rel", [(k, md, None) for k, md, _ in pb] + [(("gradB", r, e), "w", e)]))
+            comp.append(("rec", ("bwd", r, e)))
+            for c, (ev, grad, wire, par) in enumerate((("mid", "gradA", "wireA", "paramsA"), ("bwd", "gradB", "wireB", "paramsB"))):
+                comm.append(("wev", (ev, r, e)))
+                mine = [((wire, r, s), "w", None) for s in range(n)]           # the encode writes the whole chunk
+                comm.append(("acq", [((grad, r, e), "r", e)] + mine))
+                comm.append(("rel", [((grad, r, e), "r", None)] + [(k, "w", e) for k, _, _ in mine]))
+                for p in ([0] if drop == "signal_server_only" and r != 0 else [] if drop == "signal_server_only" else peers):
+                    comm.append(("sig", ("GRAD_READY", p, r), prog(e, c)))
+                for p in peers:
+                    if not (drop == "grad_ready" and c == 1 and r == 0 and p == peers[-1]):
+                        comm.append(("wait", ("GRAD_READY", r, p), prog(e, c)))
+                reads = [((wire, p, r), "r", e) for p in range(n)]           # psb_update_kernel over my shard of chunk c
+                comm.append(("acq", reads + [((par, r, p), "w", None) for p in range(n)]))
+                comm.append(("rel", [(k, md, None) for k, md, _ in reads] + [((par, r, p), "w", e) for p in range(n)]))
+            for p in range(n):
+                comm.append(("add", ("PARAMS_READY", p), 1))                  # SIGNAL_PARAMS_READY_ADD of the last launch
+            comm.append(("rec", ("done", r, e)))
+        m.add(f"r{r}.compute", comp)
+        m.add(f"r{r}.comm", comm)
+
+    def final(st, mm):
+        for p in range(n):
+            for c in ("paramsA", "paramsB"):
+                for s in range(n):
+                    v = st[2][mm.res((c, s, p))]
+                    if v != epochs:
+                        return f"rank {p} ends on {c} shard {s} version {v}, expected {epochs}"
+    m.final_checks.append(final)
+    return m
+
+
 def build_ps_unpipelined(n: int, epochs: int, drop: Optional[str] = None) -> Model:
     """``mode='ps'``, ``pipeline=False``: rank 0 gathers, updates and publishes in ONE launch inside ``step()``.
 
@@ -888,7 +949,7 @@ def build_stem_wgrad_pipeline(n: int = 1, epochs: int = 4, drop: Optional[str] =
 
 MODES = {"ps": build_ps, "ps_unpipelined": build_ps_unpipelined, "allgather": build_allgather,
          "allgather_unpipelined": build_allgather_unpipelined, "async": build_async, "stem_pipeline": build_stem_pipeline,
-         "stem_wgrad_pipeline": build_stem_wgrad_pipeline, "ps_accumulate": build_ps_accumulate}
+         "stem_wgrad_pipeline": build_stem_wgrad_pipeline, "ps_accumulate": build_ps_accumulate, "sharded": build_sharded}
 
 
 def check(mode: str, n: int, epochs: int, max_states: int = 2_000_000, **kw) -> Result:

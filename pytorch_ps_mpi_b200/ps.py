@@ -16,8 +16,9 @@ Contract kept from ``/root/reference/ps.py``:
 * ``SGD.optim_step`` / ``Adam.optim_step`` implement the reference's update math
   (``ps.py:197-214,218-261``).
 
-What is new (see DESIGN.md): three *modes* — ``'ps'`` (rank-0 parameter server: gather → sum →
-step → broadcast, the README plan ``README.md:37-46``), ``'allgather'`` (the replicated scheme
+What is new (see DESIGN.md): four *modes* — ``'ps'`` (rank-0 parameter server: gather → sum →
+step → broadcast, the README plan ``README.md:37-46``), ``'sharded'`` (the same server split over
+every rank: each gathers, steps and broadcasts its share), ``'allgather'`` (the replicated scheme
 the reference actually wires, ``ps.py:140-190``) and ``'async'`` (AsySG-InCon,
 ``README.md:56-81``) — and two *engines*: the device engine
 (:mod:`pytorch_ps_mpi_b200.parallel.device_engine`: symmetric-memory arenas + fused sm_90a
@@ -47,7 +48,7 @@ from .utils.misc import MicroBatchCounter, _bytes_of, find_param  # noqa: F401  
 
 __all__ = ["MPI_PS", "SGD", "Adam", "_bytes_of", "find_param"]
 
-_MODES = ("ps", "allgather", "async")
+_MODES = ("ps", "allgather", "async", "sharded")
 _TAG_GRAD, _TAG_PARAM = 11, 12
 
 
@@ -90,7 +91,12 @@ class MPI_PS(torch.optim.Optimizer):
 
     Parameters beyond the reference's (all keyword-only, all optional):
 
-    mode : ``'ps'`` | ``'allgather'`` | ``'async'``
+    mode : ``'ps'`` | ``'sharded'`` | ``'allgather'`` | ``'async'``
+        ``'sharded'`` computes exactly what ``'ps'`` computes, with the server's work, optimizer state and ingress split
+        evenly over all ranks (device engine: every rank serves a contiguous share of every chunk; host engine: parameter
+        ``i`` in registration order is served by rank ``i % N``).  ``state_dict()`` is then collective — call it on every
+        rank; it returns the full state everywhere, as CPU copies on the device engine — and ``opt.state[p]`` holds only the
+        step counts (the state itself stays sharded; it is not a live view as in ``'ps'``).  ``quota`` and ``consistent`` are ignored, as in ``'ps'``.
     average : divide the summed gradient by the number of contributions (default ``False`` =
         the reference's sum semantics, ``ps.py:176``)
     quota : async mode — gradients the PS consumes per update (``README.md:67-70``; default
@@ -108,7 +114,8 @@ class MPI_PS(torch.optim.Optimizer):
         before ``backward()``, and do not read parameters between ``backward()`` and ``step()``.  ``pipeline=False``
         restores one fused launch inside ``step()``.
     coalesce : host engine — ship all parameters' messages of a step as ONE framed message instead of one
-        collective per parameter (the reference's behaviour, ``ps.py:140-148``); same numerics, far fewer round trips
+        collective per parameter (the reference's behaviour, ``ps.py:140-148``); same numerics, far fewer round trips.
+        Not available with ``mode='sharded'`` (``ValueError``): its messages go to different servers.
     """
 
     _default_optim = "sgd"
@@ -132,6 +139,8 @@ class MPI_PS(torch.optim.Optimizer):
                  **kwargs):
         if mode not in _MODES:
             raise ValueError(f"mode must be one of {_MODES}")
+        if mode == "sharded" and coalesce:
+            raise ValueError("coalesce=True cannot be combined with mode='sharded' (each parameter goes to its own server)")
         self.code = code if code is not None else _codings.Identity()
         self.optim = optim if optim is not None else self._default_optim
         self.mode, self.average, self.level = mode, bool(average), int(level)
@@ -302,6 +311,8 @@ class MPI_PS(torch.optim.Optimizer):
                 data = self._step_allgather()
             elif self.mode == "ps":
                 data = self._step_ps()
+            elif self.mode == "sharded":
+                data = self._step_ps(owner=lambda i: i % self.size)
             else:
                 data = self._step_async()
             data["micro_batches"] = self._mb.n
@@ -468,7 +479,9 @@ class MPI_PS(torch.optim.Optimizer):
         return data
 
     # -- mode 'ps': rank-0 parameter server (README.md:37-46; mpi_comms.py:60-133) ----------
-    def _step_ps(self):
+    def _step_ps(self, owner=lambda i: 0):
+        """``owner(i)``: the rank serving parameter ``i`` (registration order) — rank 0 in mode 'ps', ``i % N`` in 'sharded'.
+        Each parameter is gathered to its owner, which sums and steps it; each owner then broadcasts its parameters."""
         data = {"comm_wait": 0, "optim_step_time": 0, "decode_time": 0,
                 "iallgather_prepare_time": 0.0}
         names, msgs = self._collect_encoded(data)
@@ -476,6 +489,7 @@ class MPI_PS(torch.optim.Optimizer):
         groups = self._group_of()
 
         start = time.time()
+        serves = {n: owner(i) for i, n in enumerate(self._named)}
         if self.coalesce:
             # the encoded messages travel out of band (protocol-5 buffers): no second copy into the bundle's pickle
             recv, req, _t = comms.igather({"names": names, "msgs": [pickle.PickleBuffer(m) for m in msgs]},
@@ -495,7 +509,7 @@ class MPI_PS(torch.optim.Optimizer):
             posted = []
         else:
             # one gather per parameter, all posted before any is waited (the reference's pipelining)
-            posted = [comms.igather({"name": n, "msg": pickle.PickleBuffer(m)}, name=n, level=-1)
+            posted = [comms.igather({"name": n, "msg": pickle.PickleBuffer(m)}, name=n, root=serves[n], level=-1)
                       for n, m in zip(names, msgs)]
             data["isend_time"] = time.time() - start
 
@@ -503,7 +517,7 @@ class MPI_PS(torch.optim.Optimizer):
             start = time.time()
             objs = comms.irecv(recv, req, name=n)
             data["comm_wait"] += time.time() - start
-            if self.rank != 0:
+            if self.rank != serves[n]:
                 continue
             if any(o["name"] != n for o in objs):
                 raise ValueError(f"gather order mismatch for {n}: {[o['name'] for o in objs]}")
@@ -511,16 +525,19 @@ class MPI_PS(torch.optim.Optimizer):
             grads = self._decode_all(codes, data)
             self._apply(n, grads, data, groups, scale_by=len(grads))
 
-        # PS → workers: fresh parameters (one framed message; receivers overwrite in place)
+        # PS → workers: fresh parameters (one framed message per server; receivers overwrite in place)
         start = time.time()
-        plist = [p for p in self._named.values()]
-        payload = [p.data for p in plist] if self.rank == 0 else None
-        send, req = comms.ibroadcast(payload, root=0, level=self.level)
-        fresh = comms.irecv1(send, req)
-        if self.rank != 0:
-            with torch.no_grad():
-                for p, q in zip(plist, fresh):
-                    p.data.copy_(q.to(p.device), non_blocking=True)
+        owned: Dict[int, list] = OrderedDict()
+        for n, p in self._named.items():
+            owned.setdefault(serves[n], []).append(p)
+        posted = [(r, plist, comms.ibroadcast([p.data for p in plist] if self.rank == r else None, root=r, level=self.level))
+                  for r, plist in sorted(owned.items())]
+        for r, plist, (send, req) in posted:
+            fresh = comms.irecv1(send, req)
+            if self.rank != r:
+                with torch.no_grad():
+                    for p, q in zip(plist, fresh):
+                        p.data.copy_(q.to(p.device), non_blocking=True)
         data["bcast_time"] = time.time() - start
         data["comm_wait"] += data["bcast_time"]
         return data
@@ -651,10 +668,38 @@ class MPI_PS(torch.optim.Optimizer):
                                "call step() first")
         if self._engine is not None:
             self._engine.sync_state_to_torch()
+            out = super().state_dict()
+            if self._engine.sharded:
+                self._engine.drop_state_copies()    # the returned dict keeps the full state; this rank keeps its shards only
+            return out
+        if self.mode == "sharded" and self.size > 1:
+            return self._sharded_host_state_dict()
         return super().state_dict()
+
+    def _foreign(self):
+        """mode='sharded', host engine: the parameters another rank serves (registration index mod N)."""
+        return [p for i, p in enumerate(self._named.values()) if i % self.size != self.rank]
+
+    def _sharded_host_state_dict(self):
+        """mode='sharded', host engine (collective): every owner's per-parameter state, on every rank.  The other owners'
+        state arrives as CPU copies that only the returned dict keeps."""
+        plist = list(self._named.values())
+        mine = {i: {k: v.cpu() if torch.is_tensor(v) else v for k, v in self.state[p].items()}
+                for i, p in enumerate(plist) if i % self.size == self.rank and p in self.state}
+        for theirs in runtime.world().all_gather_object(mine):
+            for i, st in theirs.items():
+                if i % self.size != self.rank:
+                    self.state[plist[i]] = st
+        out = super().state_dict()
+        for p in self._foreign():
+            self.state.pop(p, None)
+        return out
 
     def load_state_dict(self, state_dict):
         super().load_state_dict(state_dict)
+        if self._engine is None and self.mode == "sharded" and self.size > 1:
+            for p in self._foreign():               # served by another rank: its state is not kept here
+                self.state.pop(p, None)
         if self._engine is not None:
             # torch casts loaded state to the parameter dtype (bf16); the engine's state is fp32, so hand
             # it the ORIGINAL tensors, keyed by parameter position

@@ -12,3 +12,12 @@ for tool in memcheck racecheck synccheck; do
     > sanitizer_out/sanitizer_$tool.log 2>&1
   echo "exit=$?"; grep -E "ERROR SUMMARY|passed|failed|RACECHECK SUMMARY|hazard" sanitizer_out/sanitizer_$tool.log | tail -4
 done
+# mode='sharded', two ranks on one GPU (spawned processes: compute-sanitizer follows them, --target-processes all), with and
+# without the gated BcastLinear that acquires the counted PARAMS_READY
+for tool in memcheck racecheck synccheck; do
+  echo "=== compute-sanitizer --tool $tool (sharded, two ranks)"
+  timeout 1800 compute-sanitizer --tool $tool --target-processes all --error-exitcode 9 --kernel-name kernel_substring=psb_ \
+    python -m pytest tests/test_sharded_ps.py -x -q -m gpu -k "2-sgd-fp32 or bcast_linear" \
+    > sanitizer_out/sanitizer_sharded_$tool.log 2>&1
+  echo "exit=$?"; grep -E "ERROR SUMMARY|passed|failed|RACECHECK SUMMARY|hazard" sanitizer_out/sanitizer_sharded_$tool.log | tail -4
+done
