@@ -9,11 +9,12 @@ nothing goes through NCCL/MPI):
    block-wise top-k), overlapping with the rest of backward;
 2. ``step()`` raises this rank's ``GRAD_READY`` epoch flag (``st.release.sys`` into the server's
    signal pad — the ``Igatherv`` post of ``mpi_comms.py:88``);
-3. the server (rank 0 in ``mode='ps'``; every rank in ``mode='allgather'``; in ``mode='sharded'`` every rank for its own
-   share of each chunk, see ``_make_shards``) launches ``psb_update_kernel`` once: wait flags → pull every rank's wire
-   tiles over NVLink (or one ``multimem.ld_reduce`` through the switch) → decode + rank-ordered fp32 sum → SGD/Adam on fp32
-   master state → publish the new parameter tiles into every rank's *symmetric parameter
-   arena* (``multimem.st`` or peer stores) → raise ``PARAMS_READY``;
+3. every rank that serves the chunk in the static serve plan (``_make_plan``: rank 0 in ``mode='ps'``, every rank in
+   ``mode='allgather'``, every rank for its own share in ``mode='sharded'``) launches ``psb_update_kernel`` once over its
+   tiles: wait flags → pull every rank's wire tiles over NVLink (or one ``multimem.ld_reduce`` through the switch) → decode +
+   rank-ordered fp32 sum → SGD/Adam on fp32 master state → publish the new parameter tiles into every rank's *symmetric
+   parameter arena* (``multimem.st`` or peer stores; ``allgather``: its own) → the plan's completion signal on the last
+   chunk (``PARAMS_READY``; ``CONSUMED`` in ``allgather``; a counted ``PARAMS_READY`` add in ``sharded``);
 4. workers queue a one-thread wait kernel on their compute stream (the ``req.Wait()`` of
    ``mpi_comms.py:121``); the model's parameters ARE views of the parameter arena, so the next
    forward reads the fresh weights with no copy.
@@ -107,6 +108,7 @@ class DeviceEngine:
         self.wire_arena = A.tensor(self.off_wire, nt * self.bpt, torch.uint8)
         self.param_arena = A.tensor(self.off_param, n_pad * self.psz, self.dtype)
         self.stage_arena = A.tensor(self.off_stage, n_pad * self.psz, self.dtype) if self.consistent else None
+        self._sig_base = [p + self.off_signal for p in A.ptrs]
 
         # ---- move the model's parameters into the parameter arena (zero-copy from now on) ----
         with torch.no_grad():
@@ -133,10 +135,9 @@ class DeviceEngine:
 
         # ---- the pipeline chunks: contiguous runs of whole parameters in arena (= backward) order ----
         self._make_chunks()
-        self._make_shards()
+        self._make_plan()
 
-        # ---- server-side state (mode='sharded': compact, only the tiles this rank serves) ----
-        self.is_server = self.mode in ("allgather", "sharded") or self.rank == 0 or self.size == 1
+        # ---- server-side state: only the tiles this rank serves (compact in mode='sharded') ----
         self.tiles = L.tile_table_fast().to(self.device)
         self.amax = torch.zeros(max(L.nparams, 1), dtype=torch.int32, device=self.device)
         self.active_dev = torch.ones(max(L.nparams, 1), dtype=torch.uint8, device=self.device)
@@ -157,7 +158,7 @@ class DeviceEngine:
         self._mb = MicroBatchCounter()
         self.master = self.buf0 = self.buf1 = self.buf2 = None
         if self.is_server:
-            n_state = self.state_tiles * TILE if self.sharded else n_pad
+            n_state = self.state_tiles * TILE
             if self.dtype != torch.float32 and master_fp32:
                 self.master = torch.empty(n_state, dtype=torch.float32, device=self.device)
                 self._to_state(self.param_arena, self.master)
@@ -244,7 +245,6 @@ class DeviceEngine:
         # has encoded; it is saved with the optimizer state ("qsgd_step") on every rank, so a resumed run draws what a straight
         # run draws.
         self._qsgd_step = 0
-        self._sig_base = [p + self.off_signal for p in self.arena.ptrs]
         self._start_step()
         self._keep_prev: List[torch.Tensor] = []   # last step's gradients: freed one step late (see _flush)
         self._prev_done = None                      # comm-stream completion of the last step
@@ -313,9 +313,9 @@ class DeviceEngine:
         """Static chunks of the update pipeline (identical on every rank: they depend on the layout only).
 
         Chunk ``k`` = arena tiles ``[lo, hi)`` holding whole parameters, at least ``chunk_bytes`` of parameter bytes
-        each (the last one takes the remainder).  A chunk is encoded — and, on the server, gathered / updated /
-        broadcast — as soon as every parameter in it AND in all earlier chunks has produced its gradient, while
-        backward keeps running on the later chunks (``/root/reference/ps.py:140-148,159-162``: one collective per
+        each (the last one takes the remainder).  A chunk is encoded — and, by the ranks that serve it (``_make_plan``),
+        gathered / updated / published — as soon as every parameter in it AND in all earlier chunks has produced its
+        gradient, while backward keeps running on the later chunks (``/root/reference/ps.py:140-148,159-162``: one collective per
         parameter, consumed as each completes)."""
         L = self.layout
         chunks = L.plan_chunks(self.psz, self.chunk_bytes, single=(not self.pipeline and self.mode != "async"))
@@ -327,41 +327,80 @@ class DeviceEngine:
             for sl in c:
                 self._chunk_of[sl.index] = k
 
-    def _make_shards(self):
-        """``mode='sharded'``: static split of every chunk ``[lo, hi)`` into ``N`` contiguous tile ranges, one per rank in rank
-        order (identical on every rank: it depends on the layout only).  Each rank gets ``(hi - lo) // N`` tiles; the remainder
-        goes one tile each to the ``(hi - lo) % N`` ranks starting at ``k % N``, so small chunks do not all land on rank 0.
+    def _make_plan(self):
+        """The serve plan: which rank gathers, updates and publishes which tiles of every span, and how it announces that it is
+        done.  Static and identical on every rank: it depends on the layout, the mode and N only.
 
-        A rank keeps optimizer state only for its own ranges, concatenated in chunk order (``state_tiles`` tiles): the update of
-        chunk ``k`` addresses it with ``state_shift = lo_mine - compact_base``.  Tile granularity is exact for every coding: they
-        all decode per tile and read per-parameter scales and hyper-parameters by index."""
-        n = self.size
-        self.shards = []                      # per chunk: [(begin, end)] per rank
-        self._mine = []                       # per chunk: (begin, end, state_shift) of this rank
-        base = 0
+        The spans are the pipeline chunks (one span over the whole arena when not pipelined; ``async`` never is).
+        ``shards[k][r]`` is rank ``r``'s tile range ``(begin, end)`` of span ``k``, or ``None`` when ``r`` does not serve:
+
+        * ``ps`` and ``async`` (and every mode at N = 1): rank 0 serves the whole span;
+        * ``allgather``: every rank serves the whole span, publishing into its own parameter arena;
+        * ``sharded``: the span ``[lo, hi)`` is split into N contiguous ranges in rank order, ``(hi - lo) // N`` tiles each; the
+          remainder goes one tile each to the ``(hi - lo) % N`` ranks starting at ``k % N``, so small chunks do not all land on
+          rank 0.  A range may be empty.
+
+        A serving rank keeps optimizer state for its own ranges only, concatenated in span order (``state_tiles`` tiles; every
+        tile outside ``sharded``): the update of span ``k`` addresses it with ``state_shift = begin - compact_base``
+        (``_mine[k]``).  Tile granularity is exact for every coding: they all decode per tile and read per-parameter scales and
+        hyper-parameters by index."""
+        n, me = self.size, self.rank
         spans = self.chunk_tiles if self.pipeline else [(0, self.layout.ntiles)]
+        self.shards = []                      # per span: (begin, end) or None, per rank
         for k, (lo, hi) in enumerate(spans):
-            q, rem = divmod(hi - lo, n)
-            ranges, b = [], lo
-            for r in range(n):
-                e = b + q + (1 if (r - k) % n < rem else 0)
-                ranges.append((b, e))
-                b = e
+            if self.sharded:
+                q, rem = divmod(hi - lo, n)
+                ranges, b = [], lo
+                for r in range(n):
+                    e = b + q + (1 if (r - k) % n < rem else 0)
+                    ranges.append((b, e))
+                    b = e
+            elif self.mode == "allgather":
+                ranges = [(lo, hi)] * n
+            else:
+                ranges = [(lo, hi)] + [None] * (n - 1)
             self.shards.append(ranges)
-            mb, me = ranges[self.rank]
-            self._mine.append((mb, me, mb - base))
-            base += me - mb
+        self._mine = []                       # per span: (begin, end, state_shift) of this rank, or None
+        base = 0
+        for ranges in self.shards:
+            if ranges[me] is None:
+                self._mine.append(None)
+                continue
+            b, e = ranges[me]
+            self._mine.append((b, e, b - base))
+            base += e - b
         self.state_tiles = base
+        servers = [r for r in range(n) if self.shards[0][r] is not None]
+        self.is_server = me in servers
+        # GRAD_READY progress goes to the other serving ranks: a rank's own gradient is ordered by its stream.  (Async workers
+        # post their gradient to the server from _step_async.)
+        self._grad_targets = [self._sig_base[r] for r in servers if r != me] if self.mode != "async" else []
+        # The signal of a step's last launch, and what it adds to PARAMS_READY per step on a rank that another rank publishes
+        # into: that rank waits for PARAMS_READY >= epoch * _ready_per_step before its next forward (0: it waits for its own
+        # comm stream instead).
+        if n == 1:
+            self._done_signal, self._ready_per_step = SIGNAL_NONE, 0
+        elif self.mode == "ps":                       # rank 0 stores the epoch into every rank
+            self._done_signal, self._ready_per_step = SIGNAL_PARAMS_READY, 0 if self.is_server else 1
+        elif self.mode == "allgather":                # every rank publishes into its own arena
+            self._done_signal, self._ready_per_step = SIGNAL_CONSUMED, 0
+        elif self.mode == "sharded":                  # every server adds 1 into every rank
+            self._done_signal, self._ready_per_step = self.m.SIGNAL_PARAMS_READY_ADD, n
+        else:                                         # async: the server signals from _step_async, workers never wait
+            self._done_signal, self._ready_per_step = SIGNAL_PARAMS_READY, 0
 
     def _state_pieces(self, first_tile: int, ntiles: int):
         """``(arena_tile_lo, arena_tile_hi, state_tile_lo)`` for the parts of arena tiles ``[first_tile, first_tile + ntiles)``
-        whose optimizer state this rank keeps: all of them (one piece, state index = arena index) unless ``mode='sharded'``."""
-        if not self.sharded:
-            return [(first_tile, first_tile + ntiles, first_tile)]
+        whose optimizer state this (serving) rank keeps.  Pieces next to each other in the arena and in the state are merged,
+        so a rank that keeps every tile's state gets one piece (one copy in ``_to_state``)."""
         out = []
         for b, e, shift in self._mine:
             lo, hi = max(b, first_tile), min(e, first_tile + ntiles)
-            if lo < hi:
+            if lo >= hi:
+                continue
+            if out and out[-1][1] == lo and out[-1][0] - out[-1][2] == shift:
+                out[-1] = (out[-1][0], hi, out[-1][2])
+            else:
                 out.append((lo, hi, lo - shift))
         return out
 
@@ -460,10 +499,7 @@ class DeviceEngine:
                                     if k in ("step", "qsgd_step") or not torch.is_tensor(v)}
 
     def _load_slot(self, s, buf: torch.Tensor, value: torch.Tensor):
-        """Write parameter-shaped ``value`` into the state buffer ``buf`` at slot ``s`` (only this rank's tiles when sharded)."""
-        if not self.sharded:
-            s.view(buf[s.offset: s.offset + s.numel]).copy_(value.to(buf.dtype))
-            return
+        """Write parameter-shaped ``value`` into the state buffer ``buf`` at slot ``s`` (only the tiles this rank keeps)."""
         tmp = torch.zeros(s.ntiles * TILE, dtype=buf.dtype, device=buf.device)
         s.view(tmp[: s.numel]).copy_(value.to(buf.dtype))
         for lo, hi, c in self._state_pieces(s.first_tile, s.ntiles):
@@ -653,7 +689,7 @@ class DeviceEngine:
     def _flush_chunk(self, k: int, joined: bool = False, active_ptr: int = 0):
         """Everything chunk ``k`` needs, queued on the comm stream (explicit stream handle: no Python-side stream
         switching): encode its gradients into the wire arena, raise this rank's GRAD_READY progress flag from the
-        last encode CTA, and — on the server — launch the fused gather/update/broadcast kernel for exactly these tiles.
+        last encode CTA, and — on a rank that serves the span — launch the fused gather/update/publish kernel for its tiles.
 
         Must be called in chunk order.  ``joined``: the caller already made the comm stream wait for the compute stream."""
         assert k == self._next_chunk
@@ -674,15 +710,10 @@ class DeviceEngine:
             self._before_first_encode()
         epoch = self._epoch + 1
         last = k == self.nchunks - 1
-        n = self.size
-        sync = self.mode != "async"                   # async posts its flag from _step_async
-        # the launching rank's own gradient is ordered by the stream, so the server neither signals nor waits itself
-        must_signal = sync and n > 1 and not (self.mode == "ps" and self.rank == 0) and (self.pipeline or last)
+        ends_span = self.pipeline or last             # unpipelined: one span over the whole arena, after the last chunk
         sig = None
-        if must_signal:
-            sb = self._sig_base
-            targets = [sb[0]] if self.mode == "ps" else [b for r, b in enumerate(sb) if r != self.rank]
-            sig = (targets, m.SIG_GRAD_READY + self.rank, self._progress(epoch, k))
+        if self._grad_targets and ends_span:
+            sig = (self._grad_targets, m.SIG_GRAD_READY + self.rank, self._progress(epoch, k))
         items, self._chunk_items[k] = self._chunk_items[k], []
         if items:
             grads = [g for _, g in items]
@@ -703,61 +734,36 @@ class DeviceEngine:
         elif sig:                                     # nothing fired in this chunk: the flag alone
             m.signal(sig[0], sig[1], sig[2], -1, 0, csh)
             self.launches += 1
-        if self.sharded and (self.pipeline or last):
-            self._serve_shard(k if self.pipeline else 0, epoch, last, active_ptr)
-        elif sync and self.is_server and (self.pipeline or last):
-            lo, hi = self.chunk_tiles[k] if self.pipeline else (0, self.layout.ntiles)
-            inv = (1.0 / n) if self.opt.average else 1.0
-            prof = self._prof.enabled
-            ev_a = self._prof.mark(cs) if prof else None
-            wait_mask = ((1 << n) - 1) & ~(1 << self.rank)
-            if n > 1:
-                # The req.Wait() for this chunk is a ONE-WARP kernel, not the update grid: 444 update CTAs spinning on the
-                # peers' flags would hold every SM's register file (3 x 256 threads x 77 registers) while this rank's own
-                # backward still has chunks k+1.. to produce — the skew between ranks would land on the critical path.
-                m.wait_flags(self.arena.local_ptr + self.off_signal, m.SIG_GRAD_READY, wait_mask, self._progress(epoch, k),
-                             self.timeout_s, csh)
-                self.launches += 1
-            if not last or n == 1:
-                signal_mode = SIGNAL_NONE
-            else:
-                signal_mode = SIGNAL_PARAMS_READY if self.mode == "ps" else SIGNAL_CONSUMED
-            # (epoch, groups, contrib_mask, inv_count, wait_grads, signal_mode, ...)
-            self.plan.launch(epoch, self._get_hypers(), (1 << n) - 1, inv, 0, signal_mode,
-                             active_ptr=active_ptr, timeout_s=self.timeout_s,
-                             wait_mask=wait_mask, stream=csh,
-                             tile_begin=lo, tile_end=hi, wait_value=self._progress(epoch, k),
-                             param_hyper=self._phyper_ptr)
-            self.launches += 1
-            if prof:
-                self._update_spans.append((ev_a, self._prof.mark(cs)))
-
-    def _serve_shard(self, k: int, epoch: int, last: bool, active_ptr: int):
-        """``mode='sharded'``: wait for every peer's chunk-``k`` progress, then gather / update / publish this rank's share of
-        chunk ``k`` (to every rank).  The step's last launch adds 1 to every rank's PARAMS_READY instead of storing the epoch,
-        so the slot reaches ``epoch * N`` once all N servers have published; a rank with no tile in the last chunk adds its 1
-        with the signal kernel, still behind a wait for the peers' last progress value."""
-        m, csh, n = self.m, self._cs, self.size
-        lo, hi, shift = self._mine[k]
-        if hi <= lo and not last:
+        # ---- this rank's share of the span (the serve plan), for every synchronous mode; the async server launches from
+        # _step_async.  An empty share (mode='sharded') launches nothing, except the completion signal on the last chunk.
+        mine = self._mine[k if self.pipeline else 0] if ends_span and self.mode != "async" else None
+        if mine is None or (mine[0] == mine[1] and not last):
             return
+        lo, hi, shift = mine
+        n, want = self.size, self._progress(epoch, k)
         wait_mask = ((1 << n) - 1) & ~(1 << self.rank)
-        want = self._progress(epoch, k if self.pipeline else self.nchunks - 1)
-        m.wait_flags(self.arena.local_ptr + self.off_signal, m.SIG_GRAD_READY, wait_mask, want, self.timeout_s, csh)
-        self.launches += 1
-        if hi <= lo:
+        prof = self._prof.enabled and hi > lo
+        ev_a = self._prof.mark(cs) if prof else None
+        if n > 1:
+            # The req.Wait() for this chunk is a ONE-WARP kernel, not the update grid: 444 update CTAs spinning on the
+            # peers' flags would hold every SM's register file (3 x 256 threads x 77 registers) while this rank's own
+            # backward still has chunks k+1.. to produce — the skew between ranks would land on the critical path.
+            m.wait_flags(self.arena.local_ptr + self.off_signal, m.SIG_GRAD_READY, wait_mask, want, self.timeout_s, csh)
+            self.launches += 1
+        if hi == lo:                                  # only mode='sharded' has empty shares: its counted PARAMS_READY alone
             m.signal(self._sig_base, m.SIG_PARAMS_READY, 1, stream=csh, add=True)
             self.launches += 1
             return
-        prof = self._prof.enabled
-        ev_a = self._prof.mark(self.comm_stream) if prof else None
+        # (epoch, groups, contrib_mask, inv_count, wait_grads, signal_mode, ...); state_shift keeps its default, 0, unless
+        # this share's state is stored shifted
         self.plan.launch(epoch, self._get_hypers(), (1 << n) - 1, (1.0 / n) if self.opt.average else 1.0, 0,
-                         m.SIGNAL_PARAMS_READY_ADD if last else SIGNAL_NONE,
+                         self._done_signal if last else SIGNAL_NONE,
                          active_ptr=active_ptr, timeout_s=self.timeout_s, wait_mask=wait_mask, stream=csh,
-                         tile_begin=lo, tile_end=hi, wait_value=want, param_hyper=self._phyper_ptr, state_shift=shift)
+                         tile_begin=lo, tile_end=hi, wait_value=want, param_hyper=self._phyper_ptr,
+                         **({"state_shift": shift} if shift else {}))
         self.launches += 1
         if prof:
-            self._update_spans.append((ev_a, self._prof.mark(self.comm_stream)))
+            self._update_spans.append((ev_a, self._prof.mark(cs)))
 
     def _before_first_encode(self):
         """Queued on the comm stream before this step's first write into the wire arena."""
@@ -895,19 +901,13 @@ class DeviceEngine:
         done = self._event()
         done.record(cs)
         t3 = time.time()
-        if self.size > 1 and self.mode == "ps" and self.rank != 0:
-            if not self._gates:
-                # the req.Wait() of mpi_comms.py:121 — a one-thread kernel on the compute stream
-                m.wait_flags(self._sig_base[self.rank], m.SIG_PARAMS_READY, 1, epoch, self.timeout_s)
-                self.launches += 1
-            # else: the first forward GEMM (BcastLinear / the stem) acquires the flag inside its TMA producer
-        elif self.sharded:
-            # every rank, rank 0 included: the other shards arrive from peers, so `done` of this rank's comm stream is not enough
-            if not self._gates:
-                m.wait_flags(self._sig_base[self.rank], m.SIG_PARAMS_READY, 1, epoch * self.size, self.timeout_s)
-                self.launches += 1
-        else:
-            cur.wait_event(done)
+        if not self._ready_per_step:
+            cur.wait_event(done)             # nothing is published into this rank but by its own comm stream
+        elif not self._gates:
+            # the req.Wait() of mpi_comms.py:121 — a one-thread kernel on the compute stream (with a gate registered, the
+            # first forward GEMM, BcastLinear / the stem, acquires the flag inside its TMA producer instead)
+            m.wait_flags(self._sig_base[self.rank], m.SIG_PARAMS_READY, 1, epoch * self._ready_per_step, self.timeout_s)
+            self.launches += 1
         data["comm_wait"] = time.time() - t3
         data["chunks"] = self.nchunks
         if prof:
@@ -1171,14 +1171,11 @@ class DeviceEngine:
         if not self._gated():
             return 0, 0
         self._gate_epoch = self._epoch
-        return self.arena.local_ptr + self.off_signal + 8 * self.m.SIG_PARAMS_READY, self._params_ready_value()
+        return self.arena.local_ptr + self.off_signal + 8 * self.m.SIG_PARAMS_READY, self._epoch * self._ready_per_step
 
     def _gated(self) -> bool:
-        """Does the next forward have to acquire PARAMS_READY (a worker of mode='ps', every rank of mode='sharded')?"""
-        return self.size > 1 and self._epoch > 0 and (self.sharded or (self.mode == "ps" and self.rank != 0))
-
-    def _params_ready_value(self) -> int:
-        return self._epoch * self.size if self.sharded else self._epoch
+        """Does the next forward have to acquire PARAMS_READY (the serve plan: another rank publishes into this one)?"""
+        return self._ready_per_step > 0 and self._epoch > 0
 
     def ensure_params(self):
         """For forwards that bypass the gated kernel (eval mode, unsupported shapes) while a gate is registered: queue
@@ -1188,7 +1185,8 @@ class DeviceEngine:
         if self._gate_epoch == self._epoch:
             return
         self._gate_epoch = self._epoch
-        self.m.wait_flags(self._sig_base[self.rank], self.m.SIG_PARAMS_READY, 1, self._params_ready_value(), self.timeout_s)
+        self.m.wait_flags(self._sig_base[self.rank], self.m.SIG_PARAMS_READY, 1, self._epoch * self._ready_per_step,
+                          self.timeout_s)
         self.launches += 1
 
     def peer_param_ptr(self, param: torch.Tensor, rank: int) -> int:

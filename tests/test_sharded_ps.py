@@ -148,22 +148,32 @@ def _same(a, b, what):
             assert torch.equal(x, y), (what, float((x.float() - y.float()).abs().max()))
 
 
-def _check_shards(res, n, steps, pipeline=True):
-    """Every rank updated exactly its ranges, and the ranges of each chunk cover it once; the counted PARAMS_READY == e * N."""
+def _check_shards(res, n, steps, pipeline=True, mode="sharded"):
+    """Every rank updated exactly its plan ranges, with the plan's completion signal on the step's last launch, and keeps state
+    for exactly those tiles.  ``mode='sharded'``: the ranges of each chunk cover it once and the counted PARAMS_READY == e * N;
+    ``ps``: rank 0 serves whole chunks and PARAMS_READY == e; ``allgather``: every rank serves whole chunks and CONSUMED == e."""
     spans = res[0]["chunk_tiles"] if pipeline else [(0, res[0]["chunk_tiles"][-1][1])]
     for k, (lo, hi) in enumerate(spans):
-        got = sorted(tuple(r["shards"][k][q]) for q, r in enumerate(res))
-        assert got[0][0] == lo and got[-1][1] == hi and all(a[1] == b[0] for a, b in zip(got, got[1:])), (k, got)
-        sizes = [e - b for b, e in res[0]["shards"][k]]
-        assert max(sizes) - min(sizes) <= 1
+        if mode == "sharded":
+            got = sorted(tuple(r["shards"][k][q]) for q, r in enumerate(res))
+            assert got[0][0] == lo and got[-1][1] == hi and all(a[1] == b[0] for a, b in zip(got, got[1:])), (k, got)
+            sizes = [e - b for b, e in res[0]["shards"][k]]
+            assert max(sizes) - min(sizes) <= 1
+        else:
+            servers = range(n) if mode == "allgather" else [0]
+            assert [r["shards"][k][q] for q, r in enumerate(res)] == [(lo, hi) if q in servers else None for q in range(n)]
+    done = de.SIGNAL_NONE if n == 1 else {"ps": de.SIGNAL_PARAMS_READY, "allgather": de.SIGNAL_CONSUMED,
+                                          "sharded": H._EXT.SIGNAL_PARAMS_READY_ADD}[mode]
     for q, r in enumerate(res):
         ups = [(e[1], e[2], e[3]) for e in r["log"] if e[0] == "update"]
-        mine = [tuple(sh[q]) for sh in r["shards"] if sh[q][1] > sh[q][0]]
-        assert ups == [(b, e, H._EXT.SIGNAL_PARAMS_READY_ADD if (b, e) == tuple(r["shards"][-1][q]) else de.SIGNAL_NONE)
-                       for b, e in mine] * steps
-        assert r["state_tiles"] == sum(e - b for b, e in mine)
-        assert r["sig"][H.M.SIG_PARAMS_READY] == steps * n
-        if r["shards"][-1][q][1] == r["shards"][-1][q][0]:           # no tile of the last chunk: the counted signal alone
+        mine = [(sh[q], k == len(spans) - 1) for k, sh in enumerate(r["shards"]) if sh[q] is not None and sh[q][1] > sh[q][0]]
+        assert ups == [(b, e, done if last else de.SIGNAL_NONE) for (b, e), last in mine] * steps
+        assert r["state_tiles"] == sum(e - b for (b, e), _ in mine)
+        if n > 1 and mode == "allgather":
+            assert list(r["sig"][H.M.SIG_CONSUMED: H.M.SIG_CONSUMED + n]) == [steps] * n
+        elif n > 1:
+            assert r["sig"][H.M.SIG_PARAMS_READY] == steps * (n if mode == "sharded" else 1)
+        if r["shards"][-1][q] is not None and r["shards"][-1][q][1] == r["shards"][-1][q][0]:   # the counted signal alone
             assert sum(1 for e in r["log"] if e[0] == "signal" and e[1] == H.M.SIG_PARAMS_READY) == steps
 
 
@@ -188,6 +198,7 @@ def test_sharded_p2p_equals_ps_p2p(emu, n, case):
     got = _train(emu, n, "sharded", **kw)
     _same(got, want, case)
     _check_shards(got, n, 4, pipeline=kw.get("pipeline", True))
+    _check_shards(want, n, 4, pipeline=kw.get("pipeline", True), mode="ps")
     for r in got:                                   # ranks bit-identical
         for a, b in zip(r["params"], got[0]["params"]):
             assert torch.equal(a, b)
@@ -212,6 +223,26 @@ def test_compact_state_is_one_nth_of_the_arena(emu):
     assert [r["state_tiles"] for r in got] == [5, 5, 4]                  # of 14 arena tiles
     for r in got:
         assert r["buf0"] == r["state_tiles"] * TILE
+
+
+def _plan_facts(rank, w, model, opt, eng):
+    out = dict(chunk_tiles=list(eng.chunk_tiles), shards=eng.shards, state_tiles=eng.state_tiles, ntiles=eng.layout.ntiles,
+               buf0=None if eng.buf0 is None else eng.buf0.numel())
+    opt.close()
+    return out
+
+
+@pytest.mark.parametrize("mode", ["ps", "allgather", "async"])
+def test_serve_plan_and_state_size_in_the_other_modes(emu, mode):
+    """The same serve plan outside mode='sharded': a serving rank gets whole spans and holds every tile's state, a worker gets
+    ``None`` and holds none.  Read from the engines without training (an async engine trains differently)."""
+    got = _train(emu, 3, mode, optim="adam", body=_plan_facts)
+    servers = [0, 1, 2] if mode == "allgather" else [0]
+    spans = got[0]["chunk_tiles"] if mode != "async" else [(0, got[0]["ntiles"])]      # async never pipelines
+    for q, r in enumerate(got):
+        assert r["shards"] == [[sp if p in servers else None for p in range(3)] for sp in spans]
+        assert r["state_tiles"] == (r["ntiles"] if q in servers else 0)
+        assert r["buf0"] == (r["state_tiles"] * TILE if q in servers else None)
 
 
 @pytest.mark.parametrize("optim", ["sgd", "adam"])
