@@ -144,7 +144,10 @@ psb_bcast_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
       auto value = [&](int i, int col) {                  // accumulator i (at column col) → +bias → ReLU
         float v = acc[i];
         if (p.bias != nullptr && col < p.N) v += p.bias[col];
-        return p.relu ? fmaxf(v, 0.f) : v;
+        // ReLU as F.relu: NaN stays NaN.  fmaxf would return the 0; max.NaN returns NaN when an operand is NaN by the
+        // instruction's definition, so no math-mode flag can drop it, and it keeps every instantiation's register count.
+        if (p.relu) asm("max.NaN.f32 %0, %0, 0f00000000;" : "+f"(v));
+        return v;
       };
       if constexpr (EPI == 0) {
 #pragma unroll

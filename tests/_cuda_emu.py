@@ -540,9 +540,21 @@ std::vector<at::Tensor> stem_fwd(const at::Tensor& x, const at::Tensor& w2d, boo
   const int64_t N = x.size(0), H = x.size(2), W = x.size(3), OH = (H - 1) / 2 + 1, OW = (W - 1) / 2 + 1;
   TORCH_CHECK(W % 8 == 0 && W <= 256 && W >= 8, "fused stem: W must be a multiple of 8 and <= 256");
   auto a = im2col_stem(x);                                           // the REAL (emulated) patch-matrix kernel
-  auto y32 = at::matmul(a.to(at::kFloat), w2d.to(at::kFloat).t());   // [M,64], fp32 accumulators
-  at::Tensor sums = want_sums ? at::cat({y32.sum(0), (y32 * y32).sum(0)}).contiguous() : at::Tensor();
-  return {y32.to(at::kBFloat16).view({N, OH, OW, 64}).permute({0, 3, 1, 2}), sums};
+  auto y = at::matmul(a.to(at::kFloat), w2d.to(at::kFloat).t()).to(at::kBFloat16);   // [M,64]
+  at::Tensor sums;
+  if (want_sums) {   // as the kernel: Σy | Σy² of the bf16 values it stores, here as one "CTA" adding the rows in order
+    auto yf = y.to(at::kFloat).contiguous();
+    sums = at::zeros({128}, yf.options());
+    const float* v = yf.data_ptr<float>();
+    float* s = sums.data_ptr<float>();
+    for (int64_t r = 0; r < yf.size(0); ++r)
+      for (int c = 0; c < 64; ++c) {
+        const float e = v[r * 64 + c];
+        s[c] += e;
+        s[64 + c] = std::fma(e, e, s[64 + c]);
+      }
+  }
+  return {y.view({N, OH, OW, 64}).permute({0, 3, 1, 2}), sums};
 }
 
 at::Tensor stem_wgrad(const at::Tensor& x, const at::Tensor& gy) {
