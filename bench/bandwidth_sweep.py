@@ -39,7 +39,8 @@ NVLINK_DATASHEET_GBS = 450.0    # H100 SXM NVLink 4, per direction per GPU (data
 
 
 def code_of(arg: str):
-    """``--code``: identity | cast:<dtype> | scale:<dtype> | topk:<ratio> | qsgd:<levels> (block-wise QSGD)."""
+    """``--code``: identity | cast:<dtype> | scale:<dtype> | topk:<ratio> | qsgd:<levels> (block-wise QSGD) | sign | sign:noef
+    (block-wise sign with / without error feedback)."""
     kind, _, val = arg.partition(":")
     if kind == "identity":
         return ps.Identity()
@@ -47,6 +48,8 @@ def code_of(arg: str):
         return ps.TopK(ratio=float(val), values="bf16")
     if kind == "qsgd":
         return ps.QSGD(levels=int(val), blockwise=True)
+    if kind == "sign":
+        return ps.Sign(error_feedback=val != "noef")
     if kind == "scale":
         return ps.Scale(val)
     if kind == "cast":

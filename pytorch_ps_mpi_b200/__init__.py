@@ -8,9 +8,9 @@ from . import codings
 from . import mpi_comms
 from . import mpi_comms as comms
 from . import serialization
-from .codings import Coding, Identity, Cast, Scale, TopK, QSGD, SVD
+from .codings import Coding, Identity, Cast, Scale, TopK, QSGD, Sign, SVD
 from .ps import MPI_PS, Adam, SGD, _bytes_of, find_param
 
 __version__ = "0.1.0"
-__all__ = ["MPI_PS", "Adam", "SGD", "Coding", "Identity", "Cast", "Scale", "TopK", "QSGD", "SVD", "codings",
+__all__ = ["MPI_PS", "Adam", "SGD", "Coding", "Identity", "Cast", "Scale", "TopK", "QSGD", "Sign", "SVD", "codings",
            "mpi_comms", "comms", "serialization", "runtime", "find_param", "_bytes_of"]

@@ -9,7 +9,8 @@ uses exactly three members of the object passed as ``code=``:
   decoding (``ps.py:165``).
 
 This module ships that contract as :class:`Coding` plus the built-ins the framework fuses into
-its sm_90a kernels: :class:`Identity`, :class:`Cast`, :class:`Scale`, :class:`TopK`.  Each
+its sm_90a kernels: :class:`Identity`, :class:`Cast`, :class:`Scale`, :class:`TopK`, block-wise :class:`QSGD` and
+:class:`Sign`.  Each
 built-in has
 
 * a pure-PyTorch ``encode``/``decode`` (host slow path **and** the numerical oracle every CUDA
@@ -30,19 +31,20 @@ import numpy as np
 import torch
 
 __all__ = [
-    "Coding", "Identity", "Cast", "Scale", "TopK", "QSGD", "SVD", "DeviceCodeSpec", "TILE",
-    "WIRE_F32", "WIRE_BF16", "WIRE_F16", "WIRE_E4M3", "WIRE_E5M2", "WIRE_I8", "WIRE_I4",
-    "KIND_DENSE", "KIND_SCALED", "KIND_TOPK", "KIND_QSGD", "wire_dtype_of", "wire_code_of", "tile_k", "philox4x32_10",
+    "Coding", "Identity", "Cast", "Scale", "TopK", "QSGD", "Sign", "SVD", "DeviceCodeSpec", "TILE",
+    "WIRE_F32", "WIRE_BF16", "WIRE_F16", "WIRE_E4M3", "WIRE_E5M2", "WIRE_I8", "WIRE_I4", "WIRE_B1",
+    "KIND_DENSE", "KIND_SCALED", "KIND_TOPK", "KIND_QSGD", "KIND_SIGN", "wire_dtype_of", "wire_code_of", "tile_k", "philox4x32_10",
 ]
 
 #: elements per tile of the flat arena; every parameter starts on a tile boundary and the
 #: block-wise top-k selects inside one tile.  Must match ``PSB_TILE`` in csrc/kernels/common.cuh.
 TILE = 2048
 
-# wire element types (must match csrc/kernels/common.cuh); WIRE_I4 = two 4-bit codes per byte (block-wise QSGD only)
-WIRE_F32, WIRE_BF16, WIRE_F16, WIRE_E4M3, WIRE_E5M2, WIRE_I8, WIRE_I4 = 0, 1, 2, 3, 4, 5, 6
+# wire element types (must match csrc/kernels/common.cuh); WIRE_I4 = two 4-bit codes per byte (block-wise QSGD only), WIRE_B1 =
+# eight sign bits per byte (Sign only)
+WIRE_F32, WIRE_BF16, WIRE_F16, WIRE_E4M3, WIRE_E5M2, WIRE_I8, WIRE_I4, WIRE_B1 = 0, 1, 2, 3, 4, 5, 6, 7
 # coding kinds
-KIND_DENSE, KIND_SCALED, KIND_TOPK, KIND_QSGD = 0, 1, 2, 3
+KIND_DENSE, KIND_SCALED, KIND_TOPK, KIND_QSGD, KIND_SIGN = 0, 1, 2, 3, 4
 
 _WIRE_TORCH = {
     WIRE_F32: torch.float32, WIRE_BF16: torch.bfloat16, WIRE_F16: torch.float16,
@@ -84,7 +86,7 @@ def tile_k(ratio: float, valid: int) -> int:
 class DeviceCodeSpec:
     """Fixed binary wire layout of a built-in coding (consumed by the CUDA kernels)."""
 
-    kind: int                 # KIND_DENSE | KIND_SCALED | KIND_TOPK | KIND_QSGD
+    kind: int                 # KIND_DENSE | KIND_SCALED | KIND_TOPK | KIND_QSGD | KIND_SIGN
     wire: int                 # WIRE_* element type of the payload values (-1 = same as grad)
     ratio: float = 1.0        # top-k keep ratio (KIND_TOPK)
     error_feedback: bool = False
@@ -102,6 +104,8 @@ class DeviceCodeSpec:
         if self.kind == KIND_QSGD:
             # 2048 codes (int8, or int4 two per byte) + a 16-byte header: fp32 scale, 12 zero bytes
             return (TILE if self.wire == WIRE_I8 else TILE // 2) + 16
+        if self.kind == KIND_SIGN:
+            return TILE // 8 + 16           # 2048 sign bits + a 16-byte header: fp32 scale, 12 zero bytes
         w = self.resolved_wire(grad_dtype)
         esz = torch.empty((), dtype=_WIRE_TORCH[w]).element_size()
         if self.kind == KIND_TOPK:
@@ -507,6 +511,93 @@ class QSGD(Coding):
         if self.blockwise:
             return f"QSGD(levels={self.levels}, blockwise=True)"
         return f"QSGD(levels={self.levels})"
+
+
+class Sign(Coding):
+    """Block-wise scaled sign with error feedback (1-bit SGD, Seide et al. 2014; EF-SignSGD, Karimireddy et al. 2019): one bit per
+    element and one fp32 scale per ``TILE``-element block of the flattened tensor, fused into the device engine's kernels.
+
+    A wire tile is 256 payload bytes, bit ``e & 7`` of byte ``e >> 3`` the sign bit of element ``e`` (so -0 sends 1, a NaN 0), then a
+    16-byte header: the fp32 ``scale`` and 12 zero bytes (272 bytes per tile, 1/15 of a bf16 wire).  The rules (DESIGN.md, wire
+    numerics): ``p = g + residual`` over the tile's real elements ``R``; ``scale`` is the mean of ``|p|`` over ``R``, computed as
+    ``m * (sum of |p| / m) / |R|`` with ``m`` the abs-max, in the kernel's fixed order (0 when ``m == 0``, NaN when a NaN or ±Inf
+    is in ``R``, at most FLT_MAX).  ``decode`` is ``bit ? -scale : +scale`` on ``R`` and +0 elsewhere.  With ``error_feedback=True``
+    the coding keeps ``p - decode`` per parameter name and adds it to the next gradient of that name, so the compression error is
+    sent later instead of lost.
+
+    :meth:`encode` is the kernels' oracle and the host engine's path; it returns ``{"wire": uint8 [ntiles, 272], "shape": ...}``,
+    the exact bytes the device writes.  ``real`` (a boolean mask over the tile-padded span) describes a custom arena placement;
+    it defaults to ``index < numel``.
+    """
+
+    def __init__(self, error_feedback: bool = True):
+        self.error_feedback = bool(error_feedback)
+        self._residual = {}
+
+    def device_spec(self):
+        return DeviceCodeSpec(KIND_SIGN, WIRE_B1, error_feedback=self.error_feedback)
+
+    def encode(self, grad, name=None, real=None, **kwargs):
+        if self.error_feedback and name is None:
+            raise ValueError("Sign(error_feedback=True).encode needs name= (the parameter the residual belongs to)")
+        flat = grad.detach().reshape(-1).float().cpu().numpy()
+        n = flat.size
+        nt = max(1, -(-n // TILE))
+        p = np.zeros(nt * TILE, np.float32)
+        p[:n] = flat
+        if self.error_feedback and name in self._residual:
+            p = p + self._residual[name]
+        real = np.arange(nt * TILE) < n if real is None else np.asarray(real, bool).reshape(-1)
+        if real.size != nt * TILE:
+            raise ValueError(f"real must cover the {nt * TILE} tile-padded elements")
+        p, real = p.reshape(nt, TILE), real.reshape(nt, TILE)
+        with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+            bad = (real & ~np.isfinite(p)).any(axis=1)
+            m = np.where(real & np.isfinite(p), np.abs(p), np.float32(0)).max(axis=1)
+            t = np.where(real, np.abs(p) / np.where(m > 0, m, np.float32(1))[:, None], np.float32(0)).astype(np.float32)
+            # fp32 sum in the kernel's order: 8 elements per thread in index order, xor butterfly over 32 lanes, 8 warps in order
+            t = t.reshape(nt, 256, 8)
+            s = np.zeros((nt, 256), np.float32)
+            for j in range(8):
+                s = s + t[:, :, j]
+            s = s.reshape(nt, 8, 32)
+            lane = np.arange(32)
+            for off in (16, 8, 4, 2, 1):
+                s = s + s[:, :, lane ^ off]
+            tot = s[:, 0, 0]
+            for w in range(1, 8):
+                tot = tot + s[:, w, 0]
+            cnt = np.maximum(real.sum(axis=1), 1).astype(np.float32)
+            scale = (m * (tot / cnt)).astype(np.float32)
+        fmax = np.finfo(np.float32).max
+        scale = np.where(m > 0, np.minimum(scale, fmax), np.float32(0)).astype(np.float32)
+        scale = np.where(bad, np.uint32(0x7FFFFFFF).view(np.float32), scale)
+        bits = np.signbit(p) & ~np.isnan(p) & real
+        payload = np.packbits(bits.reshape(nt, TILE // 8, 8), axis=2, bitorder="little").reshape(nt, TILE // 8)
+        header = np.zeros((nt, 4), np.float32)
+        header[:, 0] = scale
+        if self.error_feedback:
+            with np.errstate(invalid="ignore"):
+                dec = np.where(bits, -scale[:, None], scale[:, None])
+                self._residual[name] = np.where(real, p - dec, np.float32(0)).astype(np.float32).reshape(-1)
+        wire = np.concatenate([payload, header.view(np.uint8)], axis=1)
+        return {"wire": torch.from_numpy(wire), "shape": tuple(grad.shape)}
+
+    def decode(self, code, cuda=False, real=None):
+        """The fp32 tensor ``bit ? -scale : +scale``; lanes outside ``real`` (default: past the tensor's end) are +0."""
+        wire = _as_tensor(code["wire"]).cpu().numpy()
+        shape = tuple(int(d) for d in code["shape"])
+        nt = wire.shape[0]
+        scale = wire[:, TILE // 8: TILE // 8 + 4].copy().view(np.float32)
+        bits = np.unpackbits(wire[:, :TILE // 8], axis=1, bitorder="little").astype(bool)
+        f = np.where(bits, -scale, scale).reshape(-1)
+        n = math.prod(shape)
+        real = np.arange(nt * TILE) < n if real is None else np.asarray(real, bool).reshape(-1)
+        f = np.where(real, f, np.float32(0)).astype(np.float32)
+        return self._place(torch.from_numpy(f[:n].copy()).reshape(shape), cuda)
+
+    def __repr__(self):
+        return f"Sign(error_feedback={self.error_feedback})"
 
 
 class SVD(Coding):

@@ -51,6 +51,14 @@ at::Tensor blob_tensor(uint64_t ptr, std::vector<int64_t> shape, at::ScalarType 
       .make_tensor();
 }
 
+// KIND_SIGN travels only as WIRE_B1 tiles of 272 bytes and needs the real-element mask (ntiles x 64 words, 16-byte aligned).
+void check_sign(const char* what, int kind, int wire, int bytes_per_tile, uint64_t real_mask) {
+  if (kind != KIND_SIGN) return;
+  const std::string w(what);
+  if (wire != WIRE_B1 || bytes_per_tile != PSB_TILE / 8 + 16) throw std::runtime_error(w + ": the sign coding needs WIRE_B1 and 272-byte tiles");
+  if (real_mask == 0 || real_mask % 16 != 0) throw std::runtime_error(w + ": the sign coding needs a 16-byte aligned real-element mask");
+}
+
 // Static part of the fused PS launch (pointers never change after the arenas are built).
 struct UpdatePlan {
   UpdateArgs a{};
@@ -65,11 +73,14 @@ struct UpdatePlan {
     a.signal_peer[r] = reinterpret_cast<uint64_t*>(signal_p);
   }
 
+  void set_real_mask(uint64_t p) { a.real_mask = reinterpret_cast<const uint32_t*>(p); }
+
   void launch(uint64_t epoch, const std::vector<std::vector<double>>& groups, uint32_t contrib_mask, double inv_count,
               int wait_grads, int signal_mode, uint32_t ack_mask, uint64_t version, uint64_t select_out,
               int average_dynamic, uint64_t active_ptr, double timeout_s, uint32_t wait_mask, uint64_t stream,
               int tile_begin, int tile_end, uint64_t wait_value, uint64_t param_hyper, int state_shift) {
     if (groups.size() > PSB_MAX_GROUPS) throw std::runtime_error("too many param groups for one launch");
+    check_sign("UpdatePlan.launch", kind, wire, a.bytes_per_tile, reinterpret_cast<uint64_t>(a.real_mask));
     for (size_t i = 0; i < groups.size(); ++i) {
       const auto& g = groups[i];
       if (g.size() != 11) throw std::runtime_error("group hyper tuple must have 11 entries");
@@ -148,7 +159,8 @@ void encode(int kind, int wire, const std::vector<at::Tensor>& grads, const std:
             const std::vector<int>& ntiles, const std::vector<int>& param_idx, uint64_t tiles_ptr, uint64_t wire_ptr,
             uint64_t scales_ptr, uint64_t amax_ptr, uint64_t residual_ptr, int bytes_per_tile, int cap, double ratio,
             const std::vector<uint64_t>& sig_targets, int sig_slot, uint64_t sig_value, uint64_t sig_counter,
-            uint64_t stream, uint64_t seed, uint32_t step, uint32_t rank, int levels, bool keep_leftover) {
+            uint64_t stream, uint64_t seed, uint32_t step, uint32_t rank, int levels, bool keep_leftover,
+            uint64_t real_mask) {
   const size_t n = grads.size();
   if (first_tile.size() != n || ntiles.size() != n || param_idx.size() != n) throw std::runtime_error("encode: length mismatch");
   if (n == 0) return;
@@ -167,6 +179,8 @@ void encode(int kind, int wire, const std::vector<at::Tensor>& grads, const std:
   a.seed = seed, a.step = step, a.rank = rank, a.levels = levels;
   if (kind == KIND_QSGD && (levels < 1 || levels > (wire == WIRE_I4 ? 7 : 127)))
     throw std::runtime_error("encode: QSGD levels out of range for the wire");
+  check_sign("encode", kind, wire, bytes_per_tile, real_mask);
+  a.real_mask = reinterpret_cast<const uint32_t*>(real_mask);
   for (size_t base = 0; base < n; base += PSB_ENCODE_MAX) {
     fill_batch(a, "encode", grads, first_tile, ntiles, param_idx, base);
     if (kind == KIND_SCALED) {
@@ -309,6 +323,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def_readwrite("grid", &UpdatePlan::grid)
       .def_readwrite("window_bytes", &UpdatePlan::window_bytes)
       .def("set_rank_ptrs", &UpdatePlan::set_rank_ptrs)
+      .def("set_real_mask", &UpdatePlan::set_real_mask, py::arg("ptr"))
       .def("configure",
            [](UpdatePlan& p, int world, int rank, int ntiles, int bytes_per_tile, int cap, int param_dt, int bcast, int reduce,
               uint64_t param_mc, uint64_t wire_mc, uint64_t param_local, uint64_t master, uint64_t buf0, uint64_t buf1,
@@ -341,7 +356,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("residual_ptr"), py::arg("bytes_per_tile"), py::arg("cap"), py::arg("ratio"),
         py::arg("sig_targets") = std::vector<uint64_t>{}, py::arg("sig_slot") = 0, py::arg("sig_value") = 0,
         py::arg("sig_counter") = 0, py::arg("stream") = 0, py::arg("seed") = 0, py::arg("step") = 0, py::arg("rank") = 0,
-        py::arg("levels") = 0, py::arg("keep_leftover") = true);
+        py::arg("levels") = 0, py::arg("keep_leftover") = true, py::arg("real_mask") = 0);
   m.def("accumulate", &accumulate, py::arg("grads"), py::arg("first_tile"), py::arg("ntiles"), py::arg("param_idx"),
         py::arg("tiles_ptr"), py::arg("carry_ptr"), py::arg("stream") = 0,
         "gradient accumulation: carry (fp32, arena-shaped) += each gradient, one launch per PSB_ENCODE_MAX gradients");

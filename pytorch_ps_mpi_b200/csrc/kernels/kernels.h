@@ -40,8 +40,11 @@ struct EncodeArgs {
   uint32_t step;
   uint32_t rank;
   int32_t levels;
-  // KIND_TOPK with a carry: leave it zero instead of keeping the leftover (accumulation without error feedback)
+  // KIND_TOPK / KIND_SIGN with a carry: leave it zero instead of keeping the leftover (accumulation without error feedback)
   int32_t drop_leftover;
+  // KIND_SIGN: ntiles x 64 words, bit e & 31 of word tile * 64 + (e >> 5) set iff element e of the tile is a real element of its
+  // parameter's arena view (16-byte aligned)
+  const uint32_t* real_mask;
 };
 
 struct UpdateArgs {
@@ -87,6 +90,7 @@ struct UpdateArgs {
   const uint64_t* select_out;          // async: device-side {mask, count, epochs…} from psb_select_kernel (or nullptr)
   int32_t average_dynamic;             // async: divide by the selected count
   unsigned long long timeout_ns;
+  const uint32_t* real_mask;           // KIND_SIGN: the real-element mask of EncodeArgs (lanes outside it decode to 0)
 };
 
 void psb_launch_absmax(cudaStream_t s, const EncodeArgs& a);

@@ -58,6 +58,20 @@ __device__ __forceinline__ float block_max(float v, float* red /*[8]*/) {
   return m;
 }
 
+// Fixed-order fp32 block sum: an xor butterfly over offsets 16, 8, 4, 2, 1 in every warp, then the 8 warp sums in index order,
+// every addition an explicit add_rn, so the device and a host build of this code (the CPU emulator) add the same way.  `red` may
+// be written again only after the caller's next barrier.
+__device__ __forceinline__ float block_sum_rn(float s, float* red /*[8]*/) {
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) s = add_rn(s, __shfl_xor_sync(0xffffffffu, s, off));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  s = red[0];
+#pragma unroll
+  for (int w = 1; w < PSB_THREADS / 32; ++w) s = add_rn(s, red[w]);
+  return s;
+}
+
 // which batch entry / arena tile does this CTA work on
 __device__ __forceinline__ void locate(const EncodeBatch& b, int cta, int& entry, int& tile) {
   int e = 0;
@@ -128,7 +142,7 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_absmax_kernel(const __grid_co
 }
 
 // ------------------------------------------------------------------------------------------
-// encode: gradient tile → wire tile (dense cast | abs-max scaled | block-wise top-k | block-wise QSGD)
+// encode: gradient tile → wire tile (dense cast | abs-max scaled | block-wise top-k | block-wise QSGD | block-wise sign)
 // ------------------------------------------------------------------------------------------
 // `saturate` = false only when the fp16 wire carries an fp16 gradient: then it is an exact copy, +-Inf included.
 template <int WIRE>
@@ -182,13 +196,7 @@ __device__ __forceinline__ void qsgd_encode_tile(const EncodeArgs& a, int tile, 
     t[j] = isfinite(g[j]) ? __fdiv_rn(fabsf(g[j]), m) : 0.f;
     s = add_rn(s, mul_rn(t[j], t[j]));
   }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) s = add_rn(s, __shfl_xor_sync(0xffffffffu, s, off));
-  if ((tid & 31) == 0) red[tid >> 5] = s;
-  __syncthreads();
-  s = red[0];
-#pragma unroll
-  for (int w = 1; w < PSB_THREADS / 32; ++w) s = add_rn(s, red[w]);
+  s = block_sum_rn(s, red);
   const float r = any ? __fsqrt_rn(s) : 1.f;   // >= 1 when any: the abs-max element contributes exactly 1
   const int levels = a.levels;
   const float lv = (float)levels;
@@ -232,6 +240,61 @@ __device__ __forceinline__ void qsgd_encode_tile(const EncodeArgs& a, int tile, 
   }
 }
 
+// Block-wise scaled sign (KIND_SIGN, WIRE_B1): one wire tile = 256 payload bytes, bit j of byte t the sign bit of element 8t + j,
+// then a 16-byte header holding the fp32 scale and 12 zero bytes.  Only the tile's real elements (a.real_mask) take part: the
+// others get bit 0 and count nowhere.  The rules are those of DESIGN.md (wire numerics); the float operations are explicit
+// round-to-nearest ones, as in the QSGD encode.  On return g holds the error-feedback residual: p - decode on the real elements,
+// 0 elsewhere.
+__device__ __forceinline__ uint32_t real_bits8(const uint32_t* mask, int tile) {   // this thread's 8 elements of the mask
+  return mask[(size_t)tile * (PSB_TILE / 32) + (threadIdx.x >> 2)] >> (8 * (threadIdx.x & 3)) & 0xffu;
+}
+
+__device__ __forceinline__ void sign_encode_tile(const EncodeArgs& a, int tile, uint8_t* wire_tile, float* g) {
+  __shared__ float red[PSB_THREADS / 32];
+  __shared__ int cnt[PSB_THREADS / 32];
+  const int tid = threadIdx.x;
+  const uint32_t real = real_bits8(a.real_mask, tile);
+  // m = abs-max over the real elements (exact, so its reduction order is free); a NaN or +-Inf among them makes it +Inf
+  float m = 0.f;
+#pragma unroll
+  for (int j = 0; j < PSB_EPT; ++j)
+    if (real >> j & 1u) m = fmaxf(m, isfinite(g[j]) ? fabsf(g[j]) : __uint_as_float(0x7f800000u));
+  m = block_max(m, red);
+  float scale;
+  if (!(m <= 3.40282346638528859811704183484516925e+38f)) {
+    scale = __uint_as_float(0x7fffffffu);   // one bit has no NaN code: the whole tile decodes to NaN
+  } else if (m == 0.f) {
+    scale = 0.f;
+  } else {
+    // scale = m * (sum of |p| / m over the real elements) / |R|: the mean magnitude, without overflow for any finite input
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < PSB_EPT; ++j)
+      if (real >> j & 1u) s = add_rn(s, __fdiv_rn(fabsf(g[j]), m));
+    int n = __popc(real);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) n += __shfl_xor_sync(0xffffffffu, n, off);
+    if ((tid & 31) == 0) cnt[tid >> 5] = n;
+    s = block_sum_rn(s, red);                // (its barrier also publishes cnt)
+    n = 0;
+#pragma unroll
+    for (int w = 0; w < PSB_THREADS / 32; ++w) n += cnt[w];
+    scale = mul_rn(m, __fdiv_rn(s, (float)n));
+    if (!(scale <= 3.40282346638528859811704183484516925e+38f)) scale = 3.40282346638528859811704183484516925e+38f;
+  }
+  // the sign bit; a NaN sends 0: adding the carry leaves a NaN's sign to the processor, and the tile decodes to NaN regardless
+  uint32_t bits = 0;
+#pragma unroll
+  for (int j = 0; j < PSB_EPT; ++j) {
+    const uint32_t u = __float_as_uint(g[j]);
+    bits |= (u >> 31 & real >> j & ((u & 0x7fffffffu) <= 0x7f800000u ? 1u : 0u)) << j;
+  }
+  wire_tile[tid] = (uint8_t)bits;
+  if (tid == 0) st_v4(wire_tile + PSB_TILE / 8, make_uint4(__float_as_uint(scale), 0u, 0u, 0u));
+#pragma unroll
+  for (int j = 0; j < PSB_EPT; ++j) g[j] = (real >> j & 1u) ? g[j] - ((bits >> j & 1u) ? -scale : scale) : 0.f;
+}
+
 // int4 wire: eight two's-complement nibbles, element j in bits [4j, 4j + 4); -8 is the NaN code
 __device__ __forceinline__ void unpack_i4x8(uint32_t w, float* f) {
 #pragma unroll
@@ -268,6 +331,8 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_co
     store_dense<WIRE>(wire_tile, q, true);
   } else if constexpr (KIND == KIND_QSGD) {
     qsgd_encode_tile<WIRE>(a, tile, wire_tile, g);
+  } else if constexpr (KIND == KIND_SIGN) {
+    sign_encode_tile(a, tile, wire_tile, g);
   } else {  // KIND_TOPK: block-wise magnitude top-k, ties → lower index, entries in index order
     __shared__ uint32_t hist[256];
     __shared__ uint32_t warp_tot[PSB_THREADS / 32];
@@ -360,8 +425,8 @@ __global__ void __launch_bounds__(PSB_THREADS) psb_encode_kernel(const __grid_co
       else reinterpret_cast<uint2*>(wire_tile)[p] = make_uint2(PSB_TILE, 0u);
     }
   }
-  if (carry) {   // the carry is consumed: error-feedback top-k keeps what the wire did not take, everything else zero
-    const bool keep = KIND == KIND_TOPK && !a.drop_leftover;
+  if (carry) {   // the carry is consumed: the error-feedback kinds keep what the wire did not carry, everything else zero
+    const bool keep = (KIND == KIND_TOPK || KIND == KIND_SIGN) && !a.drop_leftover;
     float4* r = carry8(a, tile);
     r[0] = keep ? make_float4(g[0], g[1], g[2], g[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
     r[1] = keep ? make_float4(g[4], g[5], g[6], g[7]) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -664,6 +729,49 @@ __global__ void __launch_bounds__(PSB_THREADS, 3) psb_update_kernel(const __grid
           }
         }
       }
+      apply_and_publish<OPT>(a, ti, e0, inv_count, acc, w, m, v, vm);
+    }
+  } else if constexpr (KIND == KIND_SIGN) {
+    // ---- block-wise sign over P2P: each rank's payload word holding this thread's byte and the scale in that rank's tile header,
+    // up to CH ranks in flight; +-scale summed in rank order, then every lane outside the tile's real elements set to 0, so
+    // padding, master and optimizer state stay exactly 0 ----
+    constexpr int CH = 8;
+    for (int tile = a.tile_begin + blockIdx.x; tile < a.tile_end; tile += gridDim.x) {
+      const TileInfo ti = a.tiles[tile];
+      if (a.active != nullptr && a.active[ti.param] == 0) continue;
+      const size_t e0 = (size_t)tile * PSB_TILE + tid * PSB_EPT;
+      const size_t tile_off = (size_t)tile * a.bytes_per_tile;
+      const uint32_t real = real_bits8(a.real_mask, tile);
+      float acc[PSB_EPT], w[PSB_EPT], m[PSB_EPT], v[PSB_EPT], vm[PSB_EPT];
+#pragma unroll
+      for (int j = 0; j < PSB_EPT; ++j) acc[j] = 0.f;
+      load_state<OPT>(a, ti, e0, w, m, v, vm);
+      for (int r0 = 0; r0 < a.world; r0 += CH) {
+        uint32_t q[CH];
+        float sc[CH];
+#pragma unroll
+        for (int c = 0; c < CH; ++c) {
+          const int r = r0 + c;
+          q[c] = 0u, sc[c] = 0.f;
+          if (r < a.world && (contrib >> r & 1u)) {
+            const uint8_t* p = reinterpret_cast<const uint8_t*>(a.wire[r]) + tile_off;
+            q[c] = ld_sys_u32(p + (tid & ~3));
+            sc[c] = ld_sys_f32(reinterpret_cast<const float*>(p + PSB_TILE / 8));
+          }
+        }
+#pragma unroll
+        for (int c = 0; c < CH; ++c) {       // fixed rank order → deterministic fp32 sum
+          const int r = r0 + c;
+          if (r < a.world && (contrib >> r & 1u)) {
+            const uint32_t b = q[c] >> (8 * (tid & 3));
+#pragma unroll
+            for (int j = 0; j < PSB_EPT; ++j) acc[j] += (b >> j & 1u) ? -sc[c] : sc[c];
+          }
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < PSB_EPT; ++j)
+        if (!(real >> j & 1u)) acc[j] = 0.f;
       apply_and_publish<OPT>(a, ti, e0, inv_count, acc, w, m, v, vm);
     }
   } else {
@@ -1047,7 +1155,7 @@ void psb_launch_encode(cudaStream_t s, int kind, int wire, const EncodeArgs& a) 
   ENC(KIND_DENSE, WIRE_F32) ENC(KIND_DENSE, WIRE_BF16) ENC(KIND_DENSE, WIRE_F16) ENC(KIND_DENSE, WIRE_E4M3)
   ENC(KIND_DENSE, WIRE_E5M2) ENC(KIND_SCALED, WIRE_I8) ENC(KIND_SCALED, WIRE_E4M3) ENC(KIND_SCALED, WIRE_E5M2)
   ENC(KIND_SCALED, WIRE_F16) ENC(KIND_TOPK, WIRE_F32) ENC(KIND_TOPK, WIRE_BF16)
-  ENC(KIND_QSGD, WIRE_I8) ENC(KIND_QSGD, WIRE_I4)
+  ENC(KIND_QSGD, WIRE_I8) ENC(KIND_QSGD, WIRE_I4) ENC(KIND_SIGN, WIRE_B1)
 #undef ENC
 }
 
@@ -1061,7 +1169,7 @@ void psb_launch_update(cudaStream_t s, int kind, int wire, int opt, const Update
   UPD(KIND_DENSE, WIRE_F32) UPD(KIND_DENSE, WIRE_BF16) UPD(KIND_DENSE, WIRE_F16) UPD(KIND_DENSE, WIRE_E4M3)
   UPD(KIND_DENSE, WIRE_E5M2) UPD(KIND_SCALED, WIRE_I8) UPD(KIND_SCALED, WIRE_E4M3) UPD(KIND_SCALED, WIRE_E5M2)
   UPD(KIND_SCALED, WIRE_F16) UPD(KIND_TOPK, WIRE_F32) UPD(KIND_TOPK, WIRE_BF16)
-  UPD(KIND_QSGD, WIRE_I8) UPD(KIND_QSGD, WIRE_I4)
+  UPD(KIND_QSGD, WIRE_I8) UPD(KIND_QSGD, WIRE_I4) UPD(KIND_SIGN, WIRE_B1)
 #undef UPD
 }
 

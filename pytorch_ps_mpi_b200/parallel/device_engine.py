@@ -35,7 +35,7 @@ from typing import Dict, List, Optional
 import torch
 
 from .. import runtime
-from ..codings import KIND_DENSE, KIND_QSGD, KIND_SCALED, KIND_TOPK, TILE, WIRE_BF16, WIRE_F16, WIRE_F32, wire_code_of
+from ..codings import KIND_DENSE, KIND_QSGD, KIND_SCALED, KIND_SIGN, TILE, WIRE_BF16, WIRE_F16, WIRE_F32, wire_code_of
 from ..ops import ext
 from ..utils.misc import CudaStepTimer, MicroBatchCounter
 from .layout import FlatLayout
@@ -146,10 +146,13 @@ class DeviceEngine:
         self._last_fired = None
         self.counters = torch.zeros(8, dtype=torch.int32, device=self.device)   # [0] done, [1] stats
         self.residual = None
-        if self.kind == KIND_TOPK and self.spec.error_feedback:
+        if self.spec.error_feedback:
             self.residual = torch.zeros(n_pad, dtype=torch.float32, device=self.device)
+        # the sign wire has no zero code: its kernels take part only over each tile's real elements (the lanes a parameter's arena
+        # view covers), so tile padding and a custom placement's interior padding stay exactly 0
+        self.real_mask = self._real_mask() if self.kind == KIND_SIGN else None
         # gradient accumulation (MPI_PS.no_sync): micro-batch gradients are summed in fp32 into `carry` (arena-shaped, allocated on
-        # first use; error-feedback top-k sums into its residual) by accumulate launches on the compute stream; the step's encode
+        # first use; an error-feedback coding sums into its residual) by accumulate launches on the compute stream; the step's encode
         # adds the carry to the last gradient (or to `_zeros` for a parameter that fired only inside no_sync) and zeroes it
         self.carry = None
         self._carry_ptr = 0
@@ -229,6 +232,8 @@ class DeviceEngine:
                         self.buf2.data_ptr() if self.buf2 is not None else 0,
                         self.tiles.data_ptr(), A.local_ptr + self.off_signal,
                         self.counters.data_ptr(), self.counters.data_ptr() + 4)
+            if self.kind == KIND_SIGN:
+                P.set_real_mask(self.real_mask.data_ptr())
             self.plan = P
         self.comm_stream = torch.cuda.Stream(device=self.device)
         self._cs = self.comm_stream.cuda_stream            # raw handle for explicit-stream launches
@@ -308,6 +313,17 @@ class DeviceEngine:
                     detail = f": first difference {diff[0] if diff else (len(every[0][8]), len(other[8]))}"
                 raise ValueError(f"rank {r} and rank 0 disagree on the {what[k]} ({other[k] if k < 8 else '...'} vs "
                                  f"{every[0][k] if k < 8 else '...'}){detail} — every rank must build the same model, coding and mode")
+
+    def _real_mask(self) -> torch.Tensor:
+        """``ntiles x 64`` 32-bit words, bit ``e & 31`` of word ``tile * 64 + (e >> 5)`` set iff element ``e`` of the tile lies in
+        its parameter's arena view (:meth:`ParamSlot.view`).  It depends on the layout only, so every rank builds the same one."""
+        import numpy as np
+        L = self.layout
+        real = torch.zeros(L.numel_padded, dtype=torch.bool)
+        for s in L.slots:
+            s.view(real[s.offset: s.offset + s.numel]).fill_(True)
+        words = np.packbits(real.numpy(), bitorder="little").view(np.int32)
+        return torch.empty(len(words), dtype=torch.int32, device=self.device).copy_(torch.from_numpy(words))
 
     def _make_chunks(self):
         """Static chunks of the update pipeline (identical on every rank: they depend on the layout only).
@@ -719,6 +735,8 @@ class DeviceEngine:
             grads = [g for _, g in items]
             kw = dict(seed=self.spec.seed, step=self._qsgd_step & 0xFFFFFFFF, rank=self.rank,
                       levels=self.spec.levels) if self.kind == KIND_QSGD else {}
+            if self.kind == KIND_SIGN:
+                kw["real_mask"] = self.real_mask.data_ptr()
             if self._carried:                 # an accumulated step: the encode adds the carry and zeroes it
                 kw["keep_leftover"] = self.residual is not None
             m.encode(self.kind, self.wire, grads, [s.first_tile for s, _ in items],

@@ -221,7 +221,7 @@ class MPI_PS(torch.optim.Optimizer):
             ok = len(dts) == 1 and next(iter(dts)) in (torch.float32, torch.bfloat16, torch.float16)
         if engine == "device" and not ok:
             raise ValueError("engine='device' needs CUDA parameters of one float dtype and a built-in "
-                             "coding with a device_spec() (Identity / Cast / Scale / block-wise TopK / QSGD(blockwise=True))")
+                             "coding with a device_spec() (Identity / Cast / Scale / block-wise TopK / QSGD(blockwise=True) / Sign)")
         return ok
 
     def close(self):
