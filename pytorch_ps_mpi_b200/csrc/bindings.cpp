@@ -5,6 +5,7 @@
 #include <torch/extension.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <memory>
 
@@ -81,6 +82,7 @@ struct UpdatePlan {
               int tile_begin, int tile_end, uint64_t wait_value, uint64_t param_hyper, int state_shift) {
     if (groups.size() > PSB_MAX_GROUPS) throw std::runtime_error("too many param groups for one launch");
     check_sign("UpdatePlan.launch", kind, wire, a.bytes_per_tile, reinterpret_cast<uint64_t>(a.real_mask));
+    if (opt != OPT_SGD && opt != OPT_ADAM && opt != OPT_ADAMW) throw std::runtime_error("UpdatePlan.launch: unknown optimizer");
     for (size_t i = 0; i < groups.size(); ++i) {
       const auto& g = groups[i];
       if (g.size() != 11) throw std::runtime_error("group hyper tuple must have 11 entries");
@@ -88,6 +90,9 @@ struct UpdatePlan {
       h.lr = (float)g[0], h.weight_decay = (float)g[1], h.momentum = (float)g[2], h.dampening = (float)g[3];
       h.beta1 = (float)g[4], h.beta2 = (float)g[5], h.eps = (float)g[6], h.step_size = (float)g[7];
       h.nesterov = (int)g[8], h.amsgrad = (int)g[9], h.first_step = (int)g[10], h.pad = 0;
+      // AdamW (slot layout in common.cuh): the denominator divides by c2 = fp32(sqrt(1 - β2^t))
+      if (opt == OPT_ADAMW && !(std::isfinite(h.beta1) && h.beta1 > 0.f))
+        throw std::runtime_error("UpdatePlan.launch: AdamW group tuple needs a finite bias correction c2 > 0 in entry 4");
     }
     a.epoch = epoch;
     // one chunk of the pipeline (tile_end < 0: the whole arena, waiting for the plain epoch value)
@@ -280,6 +285,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // launch modes (common.cuh); the enums are anonymous, so pybind11 needs them as plain ints
   m.attr("OPT_SGD") = (int)OPT_SGD;
   m.attr("OPT_ADAM") = (int)OPT_ADAM;
+  m.attr("OPT_ADAMW") = (int)OPT_ADAMW;
   m.attr("BCAST_LOCAL") = (int)BCAST_LOCAL;
   m.attr("BCAST_UNICAST") = (int)BCAST_UNICAST;
   m.attr("BCAST_MULTICAST") = (int)BCAST_MULTICAST;

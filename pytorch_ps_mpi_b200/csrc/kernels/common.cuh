@@ -27,7 +27,7 @@ enum : int { KIND_DENSE = 0, KIND_SCALED = 1, KIND_TOPK = 2, KIND_QSGD = 3, KIND
 // parameter / gradient dtypes
 enum : int { DT_F32 = 0, DT_BF16 = 1, DT_F16 = 2 };
 // optimizers
-enum : int { OPT_SGD = 0, OPT_ADAM = 1 };
+enum : int { OPT_SGD = 0, OPT_ADAM = 1, OPT_ADAMW = 2 };
 // how the updated parameter tile is published
 enum : int { BCAST_LOCAL = 0, BCAST_UNICAST = 1, BCAST_MULTICAST = 2 };
 // how the gradient tiles are gathered
@@ -55,6 +55,16 @@ struct __align__(16) TileInfo {
   int32_t first;   // first tile of this parameter
 };
 
+// Per-group hyper-parameters.  SGD and Adam read the slots by their names.  OPT_ADAMW (DESIGN.md, optimizer rule A1) uses the
+// same twelve slots; each fp32 scalar is computed in double on the host and rounded once:
+//   weight_decay = d  = fp32(1 - lr*λ)            the decoupled decay factor (1 when λ = 0: the decay is skipped)
+//   momentum     = a  = fp32(1 - β1)              the weight of the first moment's lerp
+//   dampening    =      fp32(1 - β2)
+//   beta1        = c2 = fp32(sqrt(1 - β2^t))      the bias correction of the second moment
+//   beta2, eps   =      fp32(β2), fp32(ε)
+//   step_size    = s  = fp32(lr / (1 - β1^t))
+//   amsgrad as Adam; lr is carried but not read; nesterov, first_step and pad are unused.
+// A per-parameter table (UpdateArgs::param_hyper) overrides {step_size, first_step} for SGD / Adam and {s, c2} for AdamW.
 struct GroupHyper {
   float lr, weight_decay, momentum, dampening;
   float beta1, beta2, eps, step_size;   // step_size = lr*sqrt(1-b2^t)/(1-b1^t) (ps.py:257-259)
@@ -307,6 +317,24 @@ PSB_HD inline float add_rn(float a, float b) {
   return __fadd_rn(a, b);
 #else
   return a + b;
+#endif
+}
+// fp32 fused multiply-add, rounded once to nearest even (host: the C library's correctly rounded fmaf).
+PSB_HD inline float fma_rn(float a, float b, float c) {
+#ifdef __CUDA_ARCH__
+  return __fmaf_rn(a, b, c);
+#else
+  return fmaf(a, b, c);
+#endif
+}
+// max that returns NaN when either operand is NaN (torch.maximum), where fmaxf would return the other operand.
+PSB_HD inline float max_nan(float a, float b) {
+#ifdef __CUDA_ARCH__
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+#else
+  return (a != a || b != b) ? a + b : (a > b ? a : b);
 #endif
 }
 // 4-byte load coherent at system scope (a peer's memory over NVLink); on the host a plain load.

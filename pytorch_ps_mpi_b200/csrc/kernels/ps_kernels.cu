@@ -495,16 +495,50 @@ __device__ __forceinline__ void apply_and_publish(const UpdateArgs& a, const Til
     // Adam step size and SGD's first-step momentum rule come from a per-parameter table
     const float2 ph = a.param_hyper[ti.param];
     h.step_size = ph.x;
-    h.first_step = ph.y != 0.f;
+    if constexpr (OPT == OPT_ADAMW) h.beta1 = ph.y;   // c2 (common.cuh)
+    else h.first_step = ph.y != 0.f;
   }
   float g[PSB_EPT];
 #pragma unroll
   for (int j = 0; j < PSB_EPT; ++j) g[j] = acc[j] * inv_count;
-  if (h.weight_decay != 0.f) {
+  if constexpr (OPT != OPT_ADAMW) {   // coupled L2 decay; AdamW decays the weight itself
+    if (h.weight_decay != 0.f) {
 #pragma unroll
-    for (int j = 0; j < PSB_EPT; ++j) g[j] = fmaf(h.weight_decay, w[j], g[j]);
+      for (int j = 0; j < PSB_EPT; ++j) g[j] = fmaf(h.weight_decay, w[j], g[j]);
+    }
   }
-  if constexpr (OPT == OPT_SGD) {   // /root/reference/ps.py:197-214
+  if constexpr (OPT == OPT_ADAMW) {   // DESIGN.md, optimizer rule A1: torch.optim.AdamW's fp32 sequence
+    // torch's lerp_(g, a): fma(a, g - m, m) for a < 0.5, fma(a - 1, g - m, g) otherwise (a - 1 is exact there)
+    const bool small = h.momentum < 0.5f;
+    const float wa = small ? h.momentum : add_rn(h.momentum, -1.f);
+#pragma unroll
+    for (int j = 0; j < PSB_EPT; ++j) {
+      if (h.weight_decay != 1.f) w[j] = mul_rn(w[j], h.weight_decay);
+      m[j] = fma_rn(wa, add_rn(g[j], -m[j]), small ? m[j] : g[j]);
+      v[j] = fma_rn(mul_rn(h.dampening, g[j]), g[j], mul_rn(v[j], h.beta2));
+    }
+#pragma unroll
+    for (int j = 0; j < PSB_EPT; ++j) {
+      float den_src = v[j];
+      if (h.amsgrad) {
+        vm[j] = max_nan(vm[j], v[j]);
+        den_src = vm[j];
+      }
+      const float den = add_rn(__fdiv_rn(__fsqrt_rn(den_src), h.beta1), h.eps);
+      w[j] = add_rn(w[j], __fdiv_rn(mul_rn(-h.step_size, m[j]), den));
+    }
+    float4* mp = reinterpret_cast<float4*>(a.buf0 + e0);
+    mp[0] = make_float4(m[0], m[1], m[2], m[3]);
+    mp[1] = make_float4(m[4], m[5], m[6], m[7]);
+    float4* vp = reinterpret_cast<float4*>(a.buf1 + e0);
+    vp[0] = make_float4(v[0], v[1], v[2], v[3]);
+    vp[1] = make_float4(v[4], v[5], v[6], v[7]);
+    if (h.amsgrad) {
+      float4* xp = reinterpret_cast<float4*>(a.buf2 + e0);
+      xp[0] = make_float4(vm[0], vm[1], vm[2], vm[3]);
+      xp[1] = make_float4(vm[4], vm[5], vm[6], vm[7]);
+    }
+  } else if constexpr (OPT == OPT_SGD) {   // /root/reference/ps.py:197-214
     if (h.momentum != 0.f) {
 #pragma unroll
       for (int j = 0; j < PSB_EPT; ++j) {
@@ -1107,6 +1141,7 @@ void launch_update_t(cudaStream_t s, const UpdateArgs& a, int grid) {
 template <int KIND, int WIRE>
 void launch_update_o(cudaStream_t s, int opt, const UpdateArgs& a, int grid) {
   if (opt == OPT_SGD) launch_update_t<KIND, WIRE, OPT_SGD>(s, a, grid);
+  else if (opt == OPT_ADAMW) launch_update_t<KIND, WIRE, OPT_ADAMW>(s, a, grid);
   else launch_update_t<KIND, WIRE, OPT_ADAM>(s, a, grid);
 }
 
@@ -1178,7 +1213,7 @@ int psb_update_max_grid(int kind, int wire, int opt) {
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   (void)kind, (void)wire, (void)opt;
-  return sms * 3;   // __launch_bounds__(256, 3): all CTAs co-resident (the completion counter needs no more)
+  return sms * 3;   // __launch_bounds__(256, 3) for every (kind, wire, opt): all CTAs co-resident (the completion counter needs no more)
 }
 
 void psb_launch_signal(cudaStream_t s, uint64_t* const* targets, int ntargets, int slot, uint64_t value,

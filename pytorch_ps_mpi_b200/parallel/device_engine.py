@@ -30,7 +30,7 @@ from __future__ import annotations
 import math
 import os
 import time
-from typing import Dict, List, Optional
+from typing import Callable, Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 
@@ -52,6 +52,64 @@ SIGNAL_NONE, SIGNAL_PARAMS_READY, SIGNAL_CONSUMED = 0, 1, 2
 
 def _align(n: int, a: int = 256) -> int:
     return (n + a - 1) // a * a
+
+
+# ---- what the engine needs to know about each optimizer (``MPI_PS.optim``) ----
+def _sgd_group(g, t):
+    return [float(g["lr"]), float(g["weight_decay"]), float(g["momentum"]), float(g["dampening"]),
+            0.0, 0.0, 0.0, 0.0, float(bool(g["nesterov"])), 0.0, float(t == 1)]
+
+
+def _adam_step_size(g, t):
+    b1, b2 = g["betas"]
+    return float(g["lr"]) * math.sqrt(1 - b2 ** t) / (1 - b1 ** t)     # ps.py:257-259
+
+
+def _adam_group(g, t):
+    b1, b2 = g["betas"]
+    return [float(g["lr"]), float(g["weight_decay"]), 0.0, 0.0, float(b1), float(b2),
+            float(g["eps"]), _adam_step_size(g, t), 0.0, float(bool(g.get("amsgrad", False))), float(t == 1)]
+
+
+def _adamw_bias(g, t):
+    """``(s, c2)`` of step ``t``: ``lr / (1 - β1^t)`` and ``sqrt(1 - β2^t)``, in double as ``torch.optim.AdamW`` forms them."""
+    b1, b2 = g["betas"]
+    return float(g["lr"]) / (1 - b1 ** t), (1 - b2 ** t) ** 0.5
+
+
+def _adamw_group(g, t):
+    """The AdamW slot layout of ``GroupHyper`` (csrc/kernels/common.cuh); the binding rounds each entry to fp32 once."""
+    b1, b2 = g["betas"]
+    lr, wd = float(g["lr"]), float(g["weight_decay"])
+    s, c2 = _adamw_bias(g, t)
+    return [lr, 1 - lr * wd, 1 - b1, 1 - b2, c2, float(b2), float(g["eps"]), s, 0.0,
+            float(bool(g.get("amsgrad", False))), 0.0]
+
+
+def _any(key):
+    return lambda groups: any(g.get(key, 0) for g in groups)
+
+
+class _OptimSpec(NamedTuple):
+    code: int                                       # psb_update_kernel's optimizer id (OPT_* of common.cuh)
+    buffers: Tuple[Tuple[str, str, Callable], ...]  # (opt.state key, engine buffer, needed(param_groups)) of the fp32 state
+    step_key: bool                                  # opt.state[p] carries "step" next to the buffers
+    group: Callable[[dict, int], List[float]]       # the group's 11-entry kernel tuple at step t
+    per_param: Callable[[dict, int], Tuple[float, float]]   # a parameter's param_hyper pair at its own step t
+    cache_key: Optional[Callable[[dict], tuple]]    # group fields the tuple depends on after step 1 (None: it changes every step)
+
+
+_ADAM_BUFFERS = (("exp_avg", "buf0", lambda groups: True), ("exp_avg_sq", "buf1", lambda groups: True),
+                 ("max_exp_avg_sq", "buf2", _any("amsgrad")))
+_OPTIMS = {
+    "sgd": _OptimSpec(OPT_SGD, (("momentum_buffer", "buf0", _any("momentum")),), False, _sgd_group,
+                      lambda g, t: (0.0, 1.0 if t == 1 else 0.0),
+                      lambda g: (g["lr"], g["weight_decay"], g["momentum"], g["dampening"], g["nesterov"])),
+    "adam": _OptimSpec(OPT_ADAM, _ADAM_BUFFERS, True, _adam_group,
+                       lambda g, t: (_adam_step_size(g, t), 1.0 if t == 1 else 0.0), None),
+    "adamw": _OptimSpec(2,                         # OPT_ADAMW (the extension exports it; tests/test_adamw.py checks)
+                        _ADAM_BUFFERS, True, _adamw_group, _adamw_bias, None),
+}
 
 
 class DeviceEngine:
@@ -160,18 +218,17 @@ class DeviceEngine:
         self._no_sync = False
         self._mb = MicroBatchCounter()
         self.master = self.buf0 = self.buf1 = self.buf2 = None
+        if opt.optim not in _OPTIMS:
+            raise ValueError(f"the device engine has no optimizer {opt.optim!r} (one of {sorted(_OPTIMS)})")
+        self.optim = _OPTIMS[opt.optim]
         if self.is_server:
             n_state = self.state_tiles * TILE
             if self.dtype != torch.float32 and master_fp32:
                 self.master = torch.empty(n_state, dtype=torch.float32, device=self.device)
                 self._to_state(self.param_arena, self.master)
-            need_b0 = opt.optim == "adam" or any(g.get("momentum", 0) != 0 for g in opt.param_groups)
-            if need_b0:
-                self.buf0 = torch.zeros(n_state, dtype=torch.float32, device=self.device)
-            if opt.optim == "adam":
-                self.buf1 = torch.zeros(n_state, dtype=torch.float32, device=self.device)
-                if any(g.get("amsgrad", False) for g in opt.param_groups):
-                    self.buf2 = torch.zeros(n_state, dtype=torch.float32, device=self.device)
+            for _key, buf, needed in self.optim.buffers:
+                if needed(opt.param_groups):
+                    setattr(self, buf, torch.zeros(n_state, dtype=torch.float32, device=self.device))
             if not self.sharded:
                 self._expose_state()
         self._group_steps = [0] * len(opt.param_groups)
@@ -216,7 +273,7 @@ class DeviceEngine:
         self.plan = None
         if self.is_server:
             P = self.m.UpdatePlan()
-            P.kind, P.wire, P.opt = self.kind, self.wire, (OPT_SGD if opt.optim == "sgd" else OPT_ADAM)
+            P.kind, P.wire, P.opt = self.kind, self.wire, self.optim.code
             P.grid = min(nt, self.m.update_max_grid(self.kind, self.wire, P.opt))
             pub = self.off_stage if self.consistent else self.off_param      # where fresh parameters are published
             for r in range(self.size):
@@ -450,20 +507,14 @@ class DeviceEngine:
     def _expose_state(self):
         """Make ``opt.state[p]`` views of the flat fp32 state (checkpoint parity, SURVEY §5)."""
         o = self.opt
+        bufs = self._state_buffers()
         for s in self.layout.slots:
             st = o.state[s.param]
             sl = slice(s.offset, s.offset + s.numel)
-            if o.optim == "sgd":
-                if self.buf0 is not None:
-                    st["momentum_buffer"] = s.view(self.buf0[sl])
-            else:
+            if self.optim.step_key:
                 st.setdefault("step", 0)
-                st["exp_avg"] = s.view(self.buf0[sl])
-                st["exp_avg_sq"] = s.view(self.buf1[sl])
-                if self.buf2 is not None:
-                    st["max_exp_avg_sq"] = s.view(self.buf2[sl])
-            if self.master is not None:
-                st["master_param"] = s.view(self.master[sl])
+            for key, buf in bufs:
+                st[key] = s.view(buf[sl])
 
     def sync_state_to_torch(self):
         o = self.opt
@@ -479,9 +530,7 @@ class DeviceEngine:
 
     def _state_buffers(self):
         """``(state key, flat fp32 buffer)`` of every optimizer-state buffer this engine keeps."""
-        o = self.opt
-        out = (("momentum_buffer", self.buf0 if o.optim == "sgd" else None), ("exp_avg", self.buf0 if o.optim == "adam" else None),
-               ("exp_avg_sq", self.buf1), ("max_exp_avg_sq", self.buf2), ("master_param", self.master))
+        out = [(key, getattr(self, buf)) for key, buf, _ in self.optim.buffers] + [("master_param", self.master)]
         return [(k, b) for k, b in out if b is not None]
 
     def _gather_state(self):
@@ -812,20 +861,13 @@ class DeviceEngine:
         return self._step_hyp
 
     def _upload_param_hypers(self) -> int:
-        """Per-parameter {step_size, first_step} for THIS step, assuming the parameter fires (tiles of parameters that do not
+        """Per-parameter {step_size, first_step} (AdamW: {s, c2}) for THIS step, assuming the parameter fires (tiles of parameters that do not
         are skipped through the active mask, so their entries are never read)."""
         o = self.opt
         slot = self._epoch % len(self._phyper_host)       # the comm stream lags the host by at most one step
         h, dev = self._phyper_host[slot], self._phyper_dev[slot]
         for sl in self.layout.slots:
-            t = self._param_steps[sl.index] + 1
-            g = o.param_groups[sl.group]
-            if o.optim == "adam":
-                b1, b2 = g["betas"]
-                h[sl.index, 0] = float(g["lr"]) * math.sqrt(1 - b2 ** t) / (1 - b1 ** t)
-            else:
-                h[sl.index, 0] = 0.0
-            h[sl.index, 1] = 1.0 if t == 1 else 0.0
+            h[sl.index, 0], h[sl.index, 1] = self.optim.per_param(o.param_groups[sl.group], self._param_steps[sl.index] + 1)
         with torch.cuda.stream(self.comm_stream):
             dev.copy_(h, non_blocking=True)
         return dev.data_ptr()
@@ -836,22 +878,15 @@ class DeviceEngine:
         for gi in range(len(o.param_groups)):
             self._group_steps[gi] += 1
         first = any(t == 1 for t in self._group_steps)
-        if o.optim == "sgd":
-            # SGD's tuple only changes with lr schedules / the first step: reuse the cached list otherwise
-            key = tuple((g["lr"], g["weight_decay"], g["momentum"], g["dampening"], g["nesterov"]) for g in o.param_groups)
+        cache_key = self.optim.cache_key
+        if cache_key is not None:
+            # a tuple that only changes with lr schedules / the first step (SGD's): reuse the cached list otherwise
+            key = tuple(cache_key(g) for g in o.param_groups)
             if not first and self._hyper_cache is not None and self._hyper_cache[0] == key:
                 return self._hyper_cache[1]
         for gi, g in enumerate(o.param_groups):
-            t = self._group_steps[gi]
-            if o.optim == "sgd":
-                out.append([float(g["lr"]), float(g["weight_decay"]), float(g["momentum"]), float(g["dampening"]),
-                            0.0, 0.0, 0.0, 0.0, float(bool(g["nesterov"])), 0.0, float(t == 1)])
-            else:
-                b1, b2 = g["betas"]
-                step_size = float(g["lr"]) * math.sqrt(1 - b2 ** t) / (1 - b1 ** t)     # ps.py:257-259
-                out.append([float(g["lr"]), float(g["weight_decay"]), 0.0, 0.0, float(b1), float(b2),
-                            float(g["eps"]), step_size, 0.0, float(bool(g.get("amsgrad", False))), float(t == 1)])
-        if o.optim == "sgd" and not first:
+            out.append(self.optim.group(g, self._group_steps[gi]))
+        if cache_key is not None and not first:
             self._hyper_cache = (key, out)
         return out
 

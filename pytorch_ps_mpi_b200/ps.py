@@ -14,7 +14,7 @@ Contract kept from ``/root/reference/ps.py``:
   in reverse registration (= backward) order and messages are paired to parameters by
   hook-firing order (``ps.py:121-123,155-156``);
 * ``SGD.optim_step`` / ``Adam.optim_step`` implement the reference's update math
-  (``ps.py:197-214,218-261``).
+  (``ps.py:197-214,218-261``).  ``AdamW`` (not in the reference) follows ``torch.optim.AdamW``.
 
 What is new (see DESIGN.md): four *modes* — ``'ps'`` (rank-0 parameter server: gather → sum →
 step → broadcast, the README plan ``README.md:37-46``), ``'sharded'`` (the same server split over
@@ -46,7 +46,7 @@ from . import mpi_comms as comms
 from . import runtime
 from .utils.misc import MicroBatchCounter, _bytes_of, find_param  # noqa: F401  (reference helpers, ps.py:25-50)
 
-__all__ = ["MPI_PS", "SGD", "Adam", "_bytes_of", "find_param"]
+__all__ = ["MPI_PS", "SGD", "Adam", "AdamW", "_bytes_of", "find_param"]
 
 _MODES = ("ps", "allgather", "async", "sharded")
 _TAG_GRAD, _TAG_PARAM = 11, 12
@@ -167,6 +167,9 @@ class MPI_PS(torch.optim.Optimizer):
         if not args and "params" not in kwargs:
             args = ([p for _, p in named_params],)
         super(MPI_PS, self).__init__(*args, **kwargs)
+        if self.optim == "adamw":
+            for g in self.param_groups:
+                self._check_adamw_group(g)
 
         self.quota = int(quota) if quota is not None else max(1, self.size - 1)
         self.recv_msgs: Dict[str, Any] = {}
@@ -215,7 +218,7 @@ class MPI_PS(torch.optim.Optimizer):
         params = [p for g in self.param_groups for p in g["params"]]
         all_cuda = bool(params) and all(p.is_cuda for p in params)
         spec = getattr(self.code, "device_spec", lambda: None)()
-        ok = all_cuda and spec is not None and self.optim in ("sgd", "adam")
+        ok = all_cuda and spec is not None and self.optim in ("sgd", "adam", "adamw")
         if ok:
             dts = {p.dtype for p in params}
             ok = len(dts) == 1 and next(iter(dts)) in (torch.float32, torch.bfloat16, torch.float16)
@@ -363,7 +366,17 @@ class MPI_PS(torch.optim.Optimizer):
             kw = {k: group[k] for k in ["betas", "weight_decay", "eps", "lr"]}
             kw["amsgrad"] = group.get("amsgrad", False)     # the reference forgot this (ps.py:185-186)
             return kw
-        raise ValueError("self.optim not in [sgd, adam]")
+        if self.optim == "adamw":
+            self._check_adamw_group(group)
+            kw = {k: group[k] for k in ["betas", "weight_decay", "eps", "lr"]}
+            kw["amsgrad"] = group.get("amsgrad", False)
+            return kw
+        raise ValueError("self.optim not in [sgd, adam, adamw]")
+
+    @staticmethod
+    def _check_adamw_group(group):
+        if group.get("maximize", False):
+            raise ValueError("AdamW: maximize=True is not supported (negate the loss instead)")
 
     def _collect_encoded(self, data):
         """Join the encode pool; returns ``(names, msgs)`` in hook-firing order (``ps.py:128-138``)."""
@@ -773,4 +786,52 @@ class Adam(MPI_PS, torch.optim.Adam):
         bias_correction1 = 1 - beta1 ** step
         bias_correction2 = 1 - beta2 ** step
         step_size = lr * math.sqrt(bias_correction2) / bias_correction1
+        p.data.addcdiv_(exp_avg, denom, value=-step_size)
+
+
+class AdamW(MPI_PS, torch.optim.AdamW):
+    """AdamW (decoupled weight decay, Loshchilov & Hutter) with ``torch.optim.AdamW``'s update and defaults
+    (``weight_decay=1e-2``).  Not in the reference; unlike :class:`Adam`, which keeps the reference's coupled decay and
+    ``sqrt(v) + eps`` formula, this is the optimizer transformer recipes expect, e.g. with biases and LayerNorm weights in
+    a ``weight_decay=0`` group.
+
+    The host engine runs torch's own op sequence per parameter, so on fp32 CPU tensors it is bit-identical to
+    ``torch.optim.AdamW(foreach=False)``.  The device engine runs the documented fp32 sequence of DESIGN.md (optimizer rule
+    A1), which differs from torch's CPU result only where torch's vectorised ``sqrt`` is not correctly rounded.
+    ``maximize=True`` raises ``ValueError``.
+    """
+
+    _default_optim = "adamw"
+
+    def optim_step(self, p, grad, amsgrad=False, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, lr=1e-3):
+        if grad.is_sparse:
+            raise RuntimeError("AdamW does not support sparse gradients")
+        state = self.state[p]
+        if len(state) == 0 or "exp_avg" not in state:
+            state["step"] = torch.tensor(0.0)
+            state["exp_avg"] = torch.zeros_like(p.data, memory_format=torch.preserve_format)
+            state["exp_avg_sq"] = torch.zeros_like(p.data, memory_format=torch.preserve_format)
+        if amsgrad and "max_exp_avg_sq" not in state:
+            state["max_exp_avg_sq"] = torch.zeros_like(p.data, memory_format=torch.preserve_format)
+        if not torch.is_tensor(state["step"]):
+            state["step"] = torch.tensor(float(state["step"]))
+        exp_avg, exp_avg_sq = state["exp_avg"], state["exp_avg_sq"]
+        beta1, beta2 = betas
+        state["step"] += 1
+        step = state["step"].item()
+        # torch.optim.AdamW (foreach=False), op for op
+        if weight_decay != 0:
+            p.data.mul_(1 - lr * weight_decay)
+        exp_avg.lerp_(grad, 1 - beta1)
+        exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
+        bias_correction1 = 1 - beta1 ** step
+        bias_correction2 = 1 - beta2 ** step
+        step_size = lr / bias_correction1
+        bias_correction2_sqrt = bias_correction2 ** 0.5
+        if amsgrad:
+            max_exp_avg_sq = state["max_exp_avg_sq"]
+            torch.maximum(max_exp_avg_sq, exp_avg_sq, out=max_exp_avg_sq)
+            denom = (max_exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps)
+        else:
+            denom = (exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps)
         p.data.addcdiv_(exp_avg, denom, value=-step_size)
