@@ -223,6 +223,95 @@ void accumulate(const std::vector<at::Tensor>& grads, const std::vector<int>& fi
   }
 }
 
+int num_sms() {
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms;
+}
+
+// A launch over arena tiles [tile_begin, tile_end) of an arena of `ntiles` tiles whose compact buffers start at tile `shift`.
+void check_tiles(const std::string& w, int ntiles, int tile_begin, int tile_end, int shift) {
+  if (tile_begin < 0 || tile_end > ntiles || tile_begin >= tile_end) throw std::runtime_error(w + ": bad tile range");
+  if (shift < 0 || shift > tile_begin) throw std::runtime_error(w + ": bad state_shift");
+}
+
+void check_dt(const std::string& w, int dt) {
+  if (dt != DT_F32 && dt != DT_BF16 && dt != DT_F16) throw std::runtime_error(w + ": unknown dtype code");
+}
+
+void check_aligned(const std::string& w, const char* what, uint64_t p) {
+  if (p % 16 != 0) throw std::runtime_error(w + ": " + what + " not 16-byte aligned");
+}
+
+// The weight average (DESIGN.md, rule E1) over one update launch's tiles, with that launch's state_shift.  `weight` is
+// 1 - decay, formed in double by the caller and rounded to fp32 here.  Async: `select_out` and `count` (2 x u64) make the
+// launch skip an iteration without contributors and decide the first average on the device.
+void ema(uint64_t master, uint64_t param, int param_dt, uint64_t ema_ptr, int ntiles, int tile_begin, int tile_end,
+         int state_shift, double weight, bool first, uint64_t select_out, uint64_t count, uint64_t stream, int sms) {
+  const std::string w("ema");
+  check_tiles(w, ntiles, tile_begin, tile_end, state_shift);
+  check_dt(w, param_dt);
+  if (ema_ptr == 0 || (master == 0 && param == 0)) throw std::runtime_error("ema: missing buffer");
+  check_aligned(w, "average", ema_ptr);
+  check_aligned(w, "master", master);
+  check_aligned(w, "parameter arena", param);
+  check_aligned(w, "counter", count);
+  const float a = (float)weight;
+  if (!(a > 0.f && a < 1.f)) throw std::runtime_error("ema: weight (1 - decay) must lie in (0, 1) in fp32");
+  EmaArgs e{};
+  e.master = reinterpret_cast<const float*>(master);
+  e.param = reinterpret_cast<const void*>(param);
+  e.ema = reinterpret_cast<float*>(ema_ptr);
+  e.param_dt = param_dt;
+  e.tile_begin = tile_begin, e.tile_end = tile_end, e.state_shift = state_shift;
+  e.weight = a;
+  e.first = first ? 1 : 0;
+  e.select_out = reinterpret_cast<const uint64_t*>(select_out);
+  e.count = reinterpret_cast<unsigned long long*>(count);
+  psb_launch_ema(pick_stream(stream), e, sms > 0 ? sms : num_sms());
+  check_launch("psb_ema_kernel launch");
+}
+
+// Publish a stored copy of tiles [tile_begin, tile_end) (fp32, or the parameter dtype; compact from tile `src_shift`) into the
+// parameter arenas with one of the update's publication modes.
+void publish(uint64_t src, int src_dt, int src_shift, int ntiles, int tile_begin, int tile_end, int param_dt, int bcast,
+             const std::vector<uint64_t>& param_dst, uint64_t param_mc, uint64_t param_local, uint64_t stream, int sms) {
+  const std::string w("publish");
+  check_tiles(w, ntiles, tile_begin, tile_end, src_shift);
+  check_dt(w, src_dt);
+  check_dt(w, param_dt);
+  if (src_dt != DT_F32 && src_dt != param_dt) throw std::runtime_error("publish: the source is fp32 or the parameter dtype");
+  if (src == 0) throw std::runtime_error("publish: missing source");
+  check_aligned(w, "source", src);
+  PublishArgs a{};
+  a.src = reinterpret_cast<const void*>(src);
+  a.src_dt = src_dt, a.src_shift = src_shift, a.param_dt = param_dt, a.bcast = bcast;
+  a.tile_begin = tile_begin, a.tile_end = tile_end;
+  if (bcast == BCAST_MULTICAST) {
+    if (param_mc == 0) throw std::runtime_error("publish: multicast needs the multicast address");
+    check_aligned(w, "multicast address", param_mc);
+    a.param_mc = reinterpret_cast<void*>(param_mc);
+  } else if (bcast == BCAST_UNICAST) {
+    if (param_dst.empty() || param_dst.size() > PSB_MAX_RANKS) throw std::runtime_error("publish: unicast needs 1.." +
+                                                                                         std::to_string(PSB_MAX_RANKS) + " arenas");
+    a.world = (int)param_dst.size();
+    for (size_t r = 0; r < param_dst.size(); ++r) {
+      if (param_dst[r] == 0) throw std::runtime_error("publish: missing parameter arena");
+      check_aligned(w, "parameter arena", param_dst[r]);
+      a.param_dst[r] = reinterpret_cast<void*>(param_dst[r]);
+    }
+  } else if (bcast == BCAST_LOCAL) {
+    if (param_local == 0) throw std::runtime_error("publish: missing parameter arena");
+    check_aligned(w, "parameter arena", param_local);
+    a.param_local = reinterpret_cast<void*>(param_local);
+  } else {
+    throw std::runtime_error("publish: unknown publication mode");
+  }
+  psb_launch_publish(pick_stream(stream), a, sms > 0 ? sms : num_sms());
+  check_launch("psb_publish_kernel launch");
+}
+
 void signal(const std::vector<uint64_t>& targets, int slot, uint64_t value, int extra_slot, uint64_t extra_value,
             uint64_t stream, uint64_t version_local, int version_slot, bool add) {
   std::vector<uint64_t*> t;
@@ -356,6 +445,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("state_shift") = 0);
 
   m.def("update_max_grid", &psb_update_max_grid);
+  m.def("num_sms", &num_sms, "the current device's SM count (the engine queries it once for the EMA / publication grids)");
   m.def("launch_count", []() { return (uint64_t)psb_launch_count(); }, "kernels of ours launched by this process so far");
   m.def("encode", &encode, py::arg("kind"), py::arg("wire"), py::arg("grads"), py::arg("first_tile"), py::arg("ntiles"),
         py::arg("param_idx"), py::arg("tiles_ptr"), py::arg("wire_ptr"), py::arg("scales_ptr"), py::arg("amax_ptr"),
@@ -366,6 +456,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("accumulate", &accumulate, py::arg("grads"), py::arg("first_tile"), py::arg("ntiles"), py::arg("param_idx"),
         py::arg("tiles_ptr"), py::arg("carry_ptr"), py::arg("stream") = 0,
         "gradient accumulation: carry (fp32, arena-shaped) += each gradient, one launch per PSB_ENCODE_MAX gradients");
+  m.def("ema", &ema, py::arg("master"), py::arg("param"), py::arg("param_dt"), py::arg("ema"), py::arg("ntiles"),
+        py::arg("tile_begin"), py::arg("tile_end"), py::arg("state_shift"), py::arg("weight"), py::arg("first"),
+        py::arg("select_out") = 0, py::arg("count") = 0, py::arg("stream") = 0, py::arg("num_sms") = 0,
+        "weight average (DESIGN.md, rule E1) over one update launch's tiles; num_sms: the device's SM count (0: query it)");
+  m.def("publish", &publish, py::arg("src"), py::arg("src_dt"), py::arg("src_shift"), py::arg("ntiles"), py::arg("tile_begin"),
+        py::arg("tile_end"), py::arg("param_dt"), py::arg("bcast"), py::arg("param_dst") = std::vector<uint64_t>{},
+        py::arg("param_mc") = 0, py::arg("param_local") = 0, py::arg("stream") = 0, py::arg("num_sms") = 0,
+        "publish stored weights (fp32 rounded once, or the parameter dtype bit for bit) into the parameter arenas");
   m.def("signal", &signal, py::arg("targets"), py::arg("slot"), py::arg("value"), py::arg("extra_slot") = -1,
         py::arg("extra_value") = 0, py::arg("stream") = 0, py::arg("version_local") = 0, py::arg("version_slot") = 0,
         py::arg("add") = false);

@@ -93,6 +93,34 @@ struct UpdateArgs {
   const uint32_t* real_mask;           // KIND_SIGN: the real-element mask of EncodeArgs (lanes outside it decode to 0)
 };
 
+// Exponential moving average of the weights (DESIGN.md, rule E1) over arena tiles [tile_begin, tile_end): ema = w at the first
+// average, else torch's lerp(ema, w, weight).  w is the fp32 master, or the parameter arena widened exactly when master is
+// nullptr.  master and ema are compact like an update launch's state (tile t at (t - state_shift) * PSB_TILE); param is
+// arena-indexed.
+struct EmaArgs {
+  const float* master;
+  const void* param;
+  float* ema;
+  int32_t param_dt;
+  int32_t tile_begin, tile_end, state_shift;
+  float weight;                 // fp32(1 - decay)
+  int32_t first;                // copy instead of lerp (ignored when count != nullptr)
+  const uint64_t* select_out;   // async: return at once when the select kernel chose no contributor (nullptr: always run)
+  unsigned long long* count;    // async: [0] averages taken so far (first = [0] == 0; the launch adds 1), [1] CTA arrivals
+};
+
+// Publication of a stored copy of the parameters over arena tiles [tile_begin, tile_end) into every rank's parameter arena,
+// with the update's publication modes: src is fp32 (rounded once to the parameter dtype) or the parameter dtype (copied bit
+// for bit).  src is compact (tile t at (t - src_shift) * PSB_TILE).
+struct PublishArgs {
+  const void* src;
+  void* param_dst[PSB_MAX_RANKS];
+  void* param_mc;
+  void* param_local;
+  int32_t src_dt, src_shift, param_dt, bcast, world;
+  int32_t tile_begin, tile_end;
+};
+
 void psb_launch_absmax(cudaStream_t s, const EncodeArgs& a);
 void psb_launch_encode(cudaStream_t s, int kind, int wire, const EncodeArgs& a);
 // gradient accumulation: residual[tile * PSB_TILE + i] += g[i] (fp32) for every tile of the batch; reads the gradients as the
@@ -118,6 +146,8 @@ void psb_launch_select(cudaStream_t s, const uint64_t* signal_local, uint64_t* c
 void psb_launch_snapshot(cudaStream_t s, const uint64_t* signal_local, const void* stage, void* shadow, void* params, size_t nbytes,
                          unsigned long long* scratch, int attempts, int num_sms);
 int psb_update_max_grid(int kind, int wire, int opt);
+void psb_launch_ema(cudaStream_t s, const EmaArgs& a, int num_sms);
+void psb_launch_publish(cudaStream_t s, const PublishArgs& a, int num_sms);
 
 // bcast_gemm.cu — wgmma / TMA GEMM whose weight tiles are gated on the PS broadcast epoch
 struct BcastGemmArgs {

@@ -483,6 +483,28 @@ __device__ __forceinline__ void decode_dense(const uint4& v0, const uint4& v1, f
   }
 }
 
+// Publish one thread's packed parameter vectors (`nv` of `out`) at byte offset `pbytes` of the parameter arena: through the
+// switch (multicast), into every rank's arena (unicast peer stores), or into this rank's own.  The publication of
+// apply_and_publish below, for psb_publish_kernel.
+__device__ __forceinline__ void publish_packed(int bcast, void* param_mc, void* const* param_dst, void* param_local, int world,
+                                               size_t pbytes, const uint4* out, int nv) {
+  if (bcast == BCAST_MULTICAST) {
+    uint8_t* p = reinterpret_cast<uint8_t*>(param_mc) + pbytes;
+    multimem_st_v4(p, out[0]);
+    if (nv == 2) multimem_st_v4(p + 16, out[1]);
+  } else if (bcast == BCAST_UNICAST) {
+    for (int r = 0; r < world; ++r) {
+      uint8_t* p = reinterpret_cast<uint8_t*>(param_dst[r]) + pbytes;
+      st_sys_v4(p, out[0]);
+      if (nv == 2) st_sys_v4(p + 16, out[1]);
+    }
+  } else {
+    uint8_t* p = reinterpret_cast<uint8_t*>(param_local) + pbytes;
+    st_v4(p, out[0]);
+    if (nv == 2) st_v4(p + 16, out[1]);
+  }
+}
+
 // Optimizer + publication for ONE tile whose summed gradient is already in `acc` (and whose state
 // `w`, `b0`, `b1`, `b2` has been loaded): the epilogue shared by every gather flavour.
 template <int OPT>
@@ -585,6 +607,7 @@ __device__ __forceinline__ void apply_and_publish(const UpdateArgs& a, const Til
   uint4 out[2];
   const int nv = pack8(a.param_dt, w, out);
   const size_t pbytes = e0 * (a.param_dt == DT_F32 ? 4 : 2);
+  // (the same stores as publish_packed; calling it here changes the SASS of the dense update kernels, so they stay inline)
   if (a.bcast == BCAST_MULTICAST) {
     uint8_t* p = reinterpret_cast<uint8_t*>(a.param_mc) + pbytes;
     multimem_st_v4(p, out[0]);
@@ -1145,6 +1168,70 @@ void launch_update_o(cudaStream_t s, int opt, const UpdateArgs& a, int grid) {
   else launch_update_t<KIND, WIRE, OPT_ADAM>(s, a, grid);
 }
 
+// ------------------------------------------------------------------------------------------
+// exponential moving average of the weights (DESIGN.md, rule E1) and the publication of stored weights (ema_weights())
+// ------------------------------------------------------------------------------------------
+// One pass over the update launch's tiles, queued right behind it: it reads what the update wrote (the master, or the published
+// parameter) and the compact fp32 average, and writes the average.  No peer access, no flag.  Padding lanes stay +0: the source
+// is +0 there and the average starts from it.
+__global__ void __launch_bounds__(PSB_THREADS) psb_ema_kernel(const __grid_constant__ EmaArgs a) {
+  if (a.select_out != nullptr && a.select_out[1] == 0) return;   // async: nothing was applied, nothing is averaged
+  const bool first = a.count != nullptr ? a.count[0] == 0 : a.first != 0;
+  // torch's lerp_(w, a): fma(a, w - e, e) for a < 0.5, fma(a - 1, w - e, w) otherwise (a - 1 is exact there)
+  const bool small = a.weight < 0.5f;
+  const float wa = small ? a.weight : add_rn(a.weight, -1.f);
+  for (int tile = a.tile_begin + blockIdx.x; tile < a.tile_end; tile += gridDim.x) {
+    const size_t e0 = (size_t)tile * PSB_TILE + threadIdx.x * PSB_EPT;
+    float w[PSB_EPT], e[PSB_EPT];
+    if (a.master != nullptr) load8_local(a.master, DT_F32, e0, w);
+    else load8_local(a.param, a.param_dt, e0, w);
+    if (!first) {
+      load8_local(a.ema, DT_F32, e0, e);
+#pragma unroll
+      for (int j = 0; j < PSB_EPT; ++j) w[j] = fma_rn(wa, add_rn(w[j], -e[j]), small ? e[j] : w[j]);
+    }
+    float4* ep = reinterpret_cast<float4*>(a.ema + e0);
+    ep[0] = make_float4(w[0], w[1], w[2], w[3]);
+    ep[1] = make_float4(w[4], w[5], w[6], w[7]);
+  }
+  if (a.count != nullptr) {
+    // async: every CTA has read count[0] before it arrives here; the last one to arrive counts this average
+    __shared__ int s_last;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      __threadfence();
+      s_last = atomicAdd(a.count + 1, 1ull) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (s_last && threadIdx.x == 0) {
+      a.count[1] = 0;
+      a.count[0] += 1;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(PSB_THREADS) psb_publish_kernel(const __grid_constant__ PublishArgs a) {
+  const int esz = a.param_dt == DT_F32 ? 4 : 2;
+  for (int tile = a.tile_begin + blockIdx.x; tile < a.tile_end; tile += gridDim.x) {
+    const size_t e0 = (size_t)tile * PSB_TILE + threadIdx.x * PSB_EPT;
+    uint4 out[2];
+    int nv;
+    if (a.src_dt == a.param_dt) {   // the saved parameters: their bits, NaN payloads included
+      const uint8_t* p = reinterpret_cast<const uint8_t*>(a.src) + e0 * esz;
+      nv = esz == 4 ? 2 : 1;
+      out[0] = ld_stream_v4(p);
+      if (nv == 2) out[1] = ld_stream_v4(p + 16);
+    } else {                        // the fp32 average, rounded once to the parameter dtype
+      float f[PSB_EPT];
+      load8_local(a.src, DT_F32, e0, f);
+      nv = pack8(a.param_dt, f, out);
+    }
+    publish_packed(a.bcast, a.param_mc, a.param_dst, a.param_local, a.world, e0 * esz, out, nv);
+  }
+}
+
+int small_grid(int tiles, int num_sms) { return std::max(1, std::min(tiles, num_sms * 8)); }
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------
@@ -1214,6 +1301,25 @@ int psb_update_max_grid(int kind, int wire, int opt) {
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   (void)kind, (void)wire, (void)opt;
   return sms * 3;   // __launch_bounds__(256, 3) for every (kind, wire, opt): all CTAs co-resident (the completion counter needs no more)
+}
+
+void psb_launch_ema(cudaStream_t s, const EmaArgs& a, int num_sms) {
+  // the compact buffers are handed over moved back by state_shift tiles, as the update's state (launch_update_t)
+  EmaArgs b = a;
+  const size_t d = (size_t)a.state_shift * PSB_TILE;
+  if (b.master) b.master -= d;
+  b.ema -= d;
+  b.state_shift = 0;
+  psb_ema_kernel<<<small_grid(a.tile_end - a.tile_begin, num_sms), PSB_THREADS, 0, s>>>(b);
+  psb_count_launch(1);
+}
+
+void psb_launch_publish(cudaStream_t s, const PublishArgs& a, int num_sms) {
+  PublishArgs b = a;
+  b.src = reinterpret_cast<const uint8_t*>(a.src) - (size_t)a.src_shift * PSB_TILE * (a.src_dt == DT_F32 ? 4 : 2);
+  b.src_shift = 0;
+  psb_publish_kernel<<<small_grid(a.tile_end - a.tile_begin, num_sms), PSB_THREADS, 0, s>>>(b);
+  psb_count_launch(1);
 }
 
 void psb_launch_signal(cudaStream_t s, uint64_t* const* targets, int ntargets, int slot, uint64_t value,

@@ -27,6 +27,7 @@ gradient before overwriting their wire arena.
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import os
 import time
@@ -37,7 +38,7 @@ import torch
 from .. import runtime
 from ..codings import KIND_DENSE, KIND_QSGD, KIND_SCALED, KIND_SIGN, TILE, WIRE_BF16, WIRE_F16, WIRE_F32, wire_code_of
 from ..ops import ext
-from ..utils.misc import CudaStepTimer, MicroBatchCounter
+from ..utils.misc import CudaStepTimer, MicroBatchCounter, raise_collectively
 from .layout import FlatLayout
 from .symmetric import SymmetricArena
 
@@ -229,8 +230,24 @@ class DeviceEngine:
             for _key, buf, needed in self.optim.buffers:
                 if needed(opt.param_groups):
                     setattr(self, buf, torch.zeros(n_state, dtype=torch.float32, device=self.device))
-            if not self.sharded:
-                self._expose_state()
+        # weight average (ema_decay, DESIGN.md rule E1): fp32, compact like the state; psb_ema_kernel runs behind every update
+        # launch over the same tiles.  `_ema_n`: averages taken (the first one copies); async counts them on the device.
+        self.ema = None
+        self._ema_on = getattr(opt, "ema_decay", None) is not None
+        self._ema_n = 0
+        self._ema_count = None
+        self._ema_weight = None
+        self._num_sms = 0
+        self._in_ema_weights = False
+        self._published = None
+        if self._ema_on and self.is_server:
+            self.ema = torch.zeros(self.state_tiles * TILE, dtype=torch.float32, device=self.device)
+            self._ema_weight = 1.0 - float(opt.ema_decay)        # in double; the binding rounds it to fp32 once
+            self._num_sms = self.m.num_sms()                       # the EMA / publication grids, queried once
+            if self.mode == "async":
+                self._ema_count = torch.zeros(2, dtype=torch.int64, device=self.device)
+        if self.is_server and not self.sharded:
+            self._expose_state()
         self._group_steps = [0] * len(opt.param_groups)
         self._hyper_cache = None
         # per-parameter step counts (the reference keeps optimizer state per parameter and skips p.grad is None,
@@ -296,6 +313,8 @@ class DeviceEngine:
         self._cs = self.comm_stream.cuda_stream            # raw handle for explicit-stream launches
         self._ev_pool = [torch.cuda.Event() for _ in range(64)]
         self._ev_i = 0
+        self._ema_src = (self.master.data_ptr() if self.master is not None else 0,
+                         0 if self.master is not None else A.local_ptr + (self.off_stage if self.consistent else self.off_param))
         self._tiles_ptr = self.tiles.data_ptr()
         self._wire_ptr = self.arena.local_ptr + self.off_wire
         self._scales_ptr = self.arena.local_ptr + self.off_scales
@@ -489,6 +508,7 @@ class DeviceEngine:
         self._keep: List[torch.Tensor] = []
         self._raw_bytes = 0
         self._first_flush_done = False
+        self._published = None
         self._step_hyp = None
         self._chunk_items: List[list] = [[] for _ in self.chunks]
         self._chunk_left = [len(c) for c in self.chunks]
@@ -523,14 +543,34 @@ class DeviceEngine:
                 o.state[s.param]["qsgd_step"] = self._qsgd_step
         if not self.is_server:
             return
+        if self.ema is not None:
+            # the last average of a step may still run on the comm stream (a rank that waits only for its own comm stream waits
+            # for the update, not for the average): the views handed out below are read on the current stream
+            torch.cuda.current_stream(self.device).wait_stream(self.comm_stream)
         for s in self.layout.slots:   # SGD too: the first-step momentum rule (ps.py:203-205) needs it on resume
             o.state[s.param]["step"] = self._param_steps[s.index] if self.mode != "async" else self._group_steps[s.group]
         if self.sharded:
             self._gather_state()
+        elif self.ema is not None:    # the average is state once it has been taken
+            taken = self._ema_taken()
+            for s in self.layout.slots:
+                if taken:
+                    o.state[s.param]["ema"] = s.view(self.ema[s.offset: s.offset + s.numel])
+                else:
+                    o.state[s.param].pop("ema", None)
 
-    def _state_buffers(self):
-        """``(state key, flat fp32 buffer)`` of every optimizer-state buffer this engine keeps."""
+    def _ema_taken(self) -> bool:
+        """Has the weight average been taken at least once?  (Async counts on the device: this synchronises.)"""
+        if self._ema_count is not None:
+            torch.cuda.current_stream(self.device).wait_stream(self.comm_stream)
+            return int(self._ema_count[0].item()) > 0
+        return self._ema_n > 0
+
+    def _state_buffers(self, ema: bool = False):
+        """``(state key, flat fp32 buffer)`` of every optimizer-state buffer this engine keeps (``ema``: and the average)."""
         out = [(key, getattr(self, buf)) for key, buf, _ in self.optim.buffers] + [("master_param", self.master)]
+        if ema:
+            out.append(("ema", self.ema))
         return [(k, b) for k, b in out if b is not None]
 
     def _gather_state(self):
@@ -539,7 +579,7 @@ class DeviceEngine:
         its dict is built (:meth:`drop_state_copies`), so only the returned dict keeps them."""
         torch.cuda.current_stream(self.device).wait_stream(self.comm_stream)
         torch.cuda.synchronize(self.device)
-        bufs = self._state_buffers()
+        bufs = self._state_buffers(ema=self.ema is not None and self._ema_taken())
         every = self.world.all_gather_object({k: b.cpu() for k, b in bufs})
         full = {k: torch.zeros(self.layout.numel_padded, dtype=torch.float32) for k, _ in bufs}
         for r, theirs in enumerate(every):
@@ -580,6 +620,26 @@ class DeviceEngine:
                 st = original.get(id(s.param), {}) if original is not None else o.state.get(s.param, {})
                 if "qsgd_step" in st:
                     self._qsgd_step = int(st["qsgd_step"])
+        if self._ema_on:
+            # the average resumes when every parameter has one; a checkpoint without it restarts it (the next step copies)
+            saved = [(s, original.get(id(s.param), {}) if original is not None else o.state.get(s.param, {}))
+                     for s in self.layout.slots]
+            have = [torch.is_tensor(st.get("ema")) for _, st in saved]
+            if any(have) and not all(have):
+                raise ValueError("the checkpoint has a weight average ('ema') for some parameters only")
+            self._ema_n = int(all(have))
+            if self.ema is not None:
+                # the loaded average must land after any average still queued on the comm stream, and before the next one
+                cur = torch.cuda.current_stream(self.device)
+                cur.wait_stream(self.comm_stream)
+                with torch.no_grad():
+                    for s, st in saved:
+                        if self._ema_n:
+                            self._load_slot(s, self.ema, st["ema"])
+                    if self._ema_count is not None:
+                        self._ema_count.fill_(0)
+                        self._ema_count[0] = self._ema_n
+                self.comm_stream.wait_stream(cur)
         if not self.is_server:
             return
         with torch.no_grad():
@@ -607,6 +667,8 @@ class DeviceEngine:
             self.drop_state_copies()
         else:
             self._expose_state()
+            for s in self.layout.slots:      # torch's cast copy of the average (state_dict() exposes the live one)
+                o.state[s.param].pop("ema", None)
 
     # ------------------------------------------------------------------------------- backward
     def grad_out(self, param: torch.nn.Parameter) -> Optional[torch.Tensor]:
@@ -630,6 +692,9 @@ class DeviceEngine:
     def on_grad(self, grad: torch.Tensor, name: str, param: torch.nn.Parameter):
         """Backward hook (``ps.py:98-101``): file the gradient under its chunk; every chunk that is now complete (in
         arena order) is encoded — and on the server gathered / updated / broadcast — right away, under backward."""
+        if self._in_ema_weights:
+            raise RuntimeError(f"parameter {name!r} got a gradient inside opt.ema_weights(): the parameters hold the average "
+                               "there; run backward() outside the block")
         s = self.layout.by_id[id(param)]
         g = grad.detach()
         # a gradient the producer already wrote into the wire arena (grad_out) has nothing to encode
@@ -829,6 +894,16 @@ class DeviceEngine:
                          tile_begin=lo, tile_end=hi, wait_value=want, param_hyper=self._phyper_ptr,
                          **({"state_shift": shift} if shift else {}))
         self.launches += 1
+        if self.ema is not None:
+            # the average of the tiles just updated, behind the update: it never delays the PARAMS_READY of the last chunk.  When
+            # it reads the fp32 master (memory only the comm stream touches), a rank that waits only for its own comm stream waits
+            # for `_published`, not for this launch; reading the parameters, it is waited for, since the user may write them
+            if last and self.master is not None:
+                self._published = self._event()
+                self._published.record(cs)
+            m.ema(*self._ema_src, self.dt, self.ema.data_ptr(), self.layout.ntiles, lo, hi, shift, self._ema_weight,
+                  self._ema_n == 0, stream=csh, num_sms=self._num_sms)
+            self.launches += 1
         if prof:
             self._update_spans.append((ev_a, self._prof.mark(cs)))
 
@@ -955,7 +1030,8 @@ class DeviceEngine:
         done.record(cs)
         t3 = time.time()
         if not self._ready_per_step:
-            cur.wait_event(done)             # nothing is published into this rank but by its own comm stream
+            # nothing is published into this rank but by its own comm stream
+            cur.wait_event(self._published if self._published is not None else done)
         elif not self._gates:
             # the req.Wait() of mpi_comms.py:121 — a one-thread kernel on the compute stream (with a gate registered, the
             # first forward GEMM, BcastLinear / the stem, acquires the flag inside its TMA producer instead)
@@ -984,6 +1060,8 @@ class DeviceEngine:
         data["micro_batches"] = self._mb.n
         self._epoch += 1
         self._qsgd_step += 1
+        if self._ema_on:
+            self._ema_n += 1
         if len(self._fired) != L.nparams:
             self._uniform_steps = False              # some parameter sat this step out: per-parameter counts diverge from now on
         for i in self._fired:
@@ -1059,7 +1137,7 @@ class DeviceEngine:
                 if self.consistent and self.rank != 0:
                     self.stage_arena.copy_(src)
                 if self.mode == "allgather":
-                    bufs = [b for b in (self.master, self.buf0, self.buf1, self.buf2) if b is not None]
+                    bufs = [b for b in (self.master, self.buf0, self.buf1, self.buf2, self.ema) if b is not None]
                     state = self.world.broadcast_object(
                         ([b.cpu() for b in bufs], self._group_steps, self._param_steps, self._uniform_steps)
                         if self.rank == 0 else None, src=0)
@@ -1072,10 +1150,77 @@ class DeviceEngine:
             torch.cuda.synchronize(self.device)
             self.world.barrier()
 
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """Collective: the parameters of every rank hold the weight average, rounded once to their dtype, inside the block, and
+        exactly their previous bits after it.
+
+        Order: the comm stream is drained and this rank's last publication acquired (PARAMS_READY), so every parameter arena
+        holds the same, final weights; a barrier; each serving rank saves its served tiles of its own arena and publishes its
+        average over them (the update's publication modes, so each rank's arena is written by the ranks that write it in a step);
+        sync and barrier, so no rank reads before every rank has published.  The exit syncs and barriers first, so no rank is
+        still reading the average when a peer writes into its arena, then publishes the saved tiles the same way, syncs and
+        barriers again.
+        PARAMS_READY and the epoch clocks do not move: a gated forward inside the block or after it finds its flag raised."""
+        if self.mode == "async":
+            raise RuntimeError("ema_weights() is not available in mode='async' (read the average through state_dict())")
+        if not self._ema_on:
+            raise RuntimeError("ema_weights() needs an optimizer built with ema_decay")
+        err = None
+        if self.accumulating:
+            err = "ema_weights() during gradient accumulation: call step() first"
+        elif self._fired or self._next_chunk:
+            err = "ema_weights() between backward() and step(): chunks of the step are in flight; call step() first"
+        elif self._ema_n == 0:
+            err = ("ema_weights(): no average has been taken yet (call step() first; after load_state_dict(), every rank must "
+                   "load a dict that carries the average, e.g. rank 0's)")
+        elif self._in_ema_weights:
+            err = "ema_weights() is already active"
+        raise_collectively(self.world, self.size, err)
+        cur = torch.cuda.current_stream(self.device)
+        cur.wait_stream(self.comm_stream)
+        if self._gated():
+            self.m.wait_flags(self._sig_base[self.rank], self.m.SIG_PARAMS_READY, 1, self._epoch * self._ready_per_step,
+                              self.timeout_s)
+            self.launches += 1
+        torch.cuda.synchronize(self.device)
+        self.world.barrier()
+        saved = None
+        if self.is_server:
+            saved = torch.empty(self.state_tiles * TILE, dtype=self.dtype, device=self.device)
+            self._to_state(self.param_arena, saved)
+        self._in_ema_weights = True
+        try:
+            self._publish(self.ema)
+            torch.cuda.synchronize(self.device)
+            self.world.barrier()
+            yield
+        finally:
+            # every rank has finished reading the average (its queued work included) before any rank writes into its arena
+            torch.cuda.synchronize(self.device)
+            self.world.barrier()
+            self._publish(saved)
+            torch.cuda.synchronize(self.device)
+            self.world.barrier()
+            self._in_ema_weights = False
+
+    def _publish(self, src: Optional[torch.Tensor]):
+        """Publish the compact ``src`` (fp32 average, or saved parameters) over this rank's served tiles into the arenas."""
+        if not self.is_server:
+            return
+        A = self.arena
+        dst = [p + self.off_param for p in A.ptrs] if self.bcast == BCAST_UNICAST else []
+        mc = A.mc_ptr + self.off_param if self.bcast == BCAST_MULTICAST else 0
+        for lo, hi, c in self._state_pieces(0, self.layout.ntiles):
+            self.m.publish(src.data_ptr(), _DT[src.dtype], lo - c, self.layout.ntiles, lo, hi, self.dt, self.bcast, dst, mc,
+                           A.local_ptr + self.off_param, num_sms=self._num_sms)
+            self.launches += 1
+
     def resync_master(self):
         """Re-seed the fp32 master weights from the (bf16/fp16) parameters — call after changing parameters in place
-        behind the optimizer's back (``model.load_state_dict`` without ``opt.load_state_dict``, manual re-init, EMA
-        swaps): every update writes master → parameters, so un-synced edits would be overwritten."""
+        behind the optimizer's back (``model.load_state_dict`` without ``opt.load_state_dict``, manual re-init; evaluating
+        with the weight average needs none of this: :meth:`ema_weights`): every update writes master → parameters, so
+        un-synced edits would be overwritten."""
         if self.master is not None:
             torch.cuda.current_stream(self.device).wait_stream(self.comm_stream)
             with torch.no_grad():
@@ -1137,6 +1282,14 @@ class DeviceEngine:
         with torch.cuda.stream(cs):
             slot["host"].copy_(self._select_out, non_blocking=True)
         slot["event"].record(cs)
+        if self.ema is not None:
+            # once per applied update: the select's count gates it, the device counts the first.  Queued behind the slot's event,
+            # so harvesting an iteration waits for its update, not for the average
+            L = self.layout
+            self.m.ema(*self._ema_src, self.dt, self.ema.data_ptr(), L.ntiles, 0, L.ntiles, 0, self._ema_weight, False,
+                       select_out=self._select_out.data_ptr(), count=self._ema_count.data_ptr(), stream=self._cs,
+                       num_sms=self._num_sms)
+            self.launches += 1
         slot["version"] = self.version
         self._async_pending.append(slot)
         if len(self._async_pending) >= self._async_depth:

@@ -44,7 +44,8 @@ import torch
 from . import codings as _codings
 from . import mpi_comms as comms
 from . import runtime
-from .utils.misc import MicroBatchCounter, _bytes_of, find_param  # noqa: F401  (reference helpers, ps.py:25-50)
+from .utils.misc import MicroBatchCounter, raise_collectively
+from .utils.misc import _bytes_of, find_param  # noqa: F401  (reference helpers, ps.py:25-50)
 
 __all__ = ["MPI_PS", "SGD", "Adam", "AdamW", "_bytes_of", "find_param"]
 
@@ -116,6 +117,15 @@ class MPI_PS(torch.optim.Optimizer):
     coalesce : host engine — ship all parameters' messages of a step as ONE framed message instead of one
         collective per parameter (the reference's behaviour, ``ps.py:140-148``); same numerics, far fewer round trips.
         Not available with ``mode='sharded'`` (``ValueError``): its messages go to different servers.
+    ema_decay : keep an exponential moving average of the weights (EMA, Polyak averaging) with this decay, in ``(0, 1)``;
+        ``None`` (default) keeps none.  The semantics are those of ``torch.optim.swa_utils.AveragedModel(model,
+        multi_avg_fn=get_ema_multi_avg_fn(ema_decay))`` with ``update_parameters()`` after every ``step()``: the first step
+        copies the weights, every later one does ``ema.lerp_(w, 1 - ema_decay)``, for every parameter the optimizer holds,
+        including parameters that got no gradient in that step.  Buffers (BatchNorm running statistics) are not averaged,
+        as in torch's default.  The rank that applies a parameter's update keeps the average in fp32, from the fp32 master
+        weights where there are any (DESIGN.md, rule E1); on the device engine it is updated on the server's stream, under
+        backward.  ``state_dict()`` carries it as the per-parameter state ``ema``; use the average for evaluation with
+        :meth:`ema_weights`.  In ``mode='async'`` the server averages after each update it applies.
     """
 
     _default_optim = "sgd"
@@ -136,9 +146,14 @@ class MPI_PS(torch.optim.Optimizer):
                  reduce: str = "auto",
                  coalesce: bool = False,
                  pipeline: bool = True,
+                 ema_decay: Optional[float] = None,
                  **kwargs):
         if mode not in _MODES:
             raise ValueError(f"mode must be one of {_MODES}")
+        if ema_decay is not None and not (isinstance(ema_decay, (int, float)) and 0.0 < float(ema_decay) < 1.0):
+            raise ValueError(f"ema_decay must lie in (0, 1), got {ema_decay!r}")
+        self.ema_decay = None if ema_decay is None else float(ema_decay)
+        self._in_ema_weights = False
         if mode == "sharded" and coalesce:
             raise ValueError("coalesce=True cannot be combined with mode='sharded' (each parameter goes to its own server)")
         self.code = code if code is not None else _codings.Identity()
@@ -266,6 +281,9 @@ class MPI_PS(torch.optim.Optimizer):
         """Backward hook: queue the encode on the pool and remember hook-firing order (``ps.py:98-101``).  Inside ``no_sync()``
         the gradient is added to the name's fp32 carry instead; the next gradient of that name is sent as (carry + gradient),
         rounded once to the gradient's dtype."""
+        if self._in_ema_weights:
+            raise RuntimeError(f"parameter {name!r} got a gradient inside opt.ema_weights(): the parameters hold the average "
+                               "there; run backward() outside the block")
         self._mb.fire(name)
         if self._no_sync:
             self._accumulated = True
@@ -299,6 +317,8 @@ class MPI_PS(torch.optim.Optimizer):
         """Perform one optimization step; returns ``(loss, data)`` (``ps.py:103-193``)."""
         if self._no_sync:
             raise RuntimeError("step() inside no_sync(): leave the no_sync() block first (its gradients are summed, not sent)")
+        if self._in_ema_weights:
+            raise RuntimeError("step() inside ema_weights(): the parameters hold the average there; leave the block first")
         loss = None
         if closure is not None:
             with torch.enable_grad():
@@ -318,6 +338,8 @@ class MPI_PS(torch.optim.Optimizer):
                 data = self._step_ps(owner=lambda i: i % self.size)
             else:
                 data = self._step_async()
+            if self.ema_decay is not None and (self.mode != "async" or self.size == 1 or data.get("contributors")):
+                self._host_ema_update(self._ema_params())
             data["micro_batches"] = self._mb.n
             self._mb.reset()
             self._accumulated = False
@@ -357,6 +379,88 @@ class MPI_PS(torch.optim.Optimizer):
             self._mb.cut()
             if self._engine is not None:
                 self._engine.end_no_sync()
+
+    # -- weight average (ema_decay) ------------------------------------------------------------
+    def _ema_params(self, rank=None):
+        """Host engine: the parameters whose update ``rank`` (default: this rank) applies, so whose average it keeps."""
+        rank = self.rank if rank is None else rank
+        plist = list(self._named.values())
+        if self.mode == "allgather" or self.size == 1:
+            return plist
+        if self.mode == "sharded":
+            return [p for i, p in enumerate(plist) if i % self.size == rank]
+        return plist if rank == 0 else []
+
+    def _host_ema_update(self, params):
+        """``AveragedModel.update_parameters`` on fp32 copies: a parameter without an average copies, the others lerp."""
+        with torch.no_grad():
+            old = [p for p in params if "ema" in self.state[p]]
+            for p in params:
+                if "ema" not in self.state[p]:
+                    self.state[p]["ema"] = p.detach().to(torch.float32, copy=True)
+            if old:
+                torch._foreach_lerp_([self.state[p]["ema"] for p in old], [p.detach().float() for p in old],
+                                     1.0 - self.ema_decay)
+
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """Evaluate with the weight average (``ema_decay``)::
+
+            with opt.ema_weights():          # every rank: the parameters hold the average
+                model.eval()
+                accuracy = evaluate(model)
+            model.train()                    # the parameters are bit for bit what they were; training goes on
+
+        Collective in the synchronous modes (``'ps'``, ``'sharded'``, ``'allgather'``): call it on every rank, between a
+        ``step()`` and the next ``backward()``.  Inside the block every rank's parameters hold the average rounded once to
+        their dtype; on exit they hold exactly their previous bits, and training continues as if the block had never been
+        entered.  Buffers are not averaged.  Raises in ``mode='async'`` (read the average through ``state_dict()``), while
+        gradients are accumulated and not sent, and between a ``backward()`` and its ``step()``; a gradient or a ``step()``
+        inside the block raises too."""
+        if self.ema_decay is None:
+            raise RuntimeError("ema_weights() needs an optimizer built with ema_decay")
+        if self._in_ema_weights:
+            raise RuntimeError("ema_weights() is already active")
+        if self._engine is not None:
+            with self._engine.ema_weights():
+                self._in_ema_weights = True
+                try:
+                    yield
+                finally:
+                    self._in_ema_weights = False
+            return
+        if self.mode == "async" and self.size > 1:
+            raise RuntimeError("ema_weights() is not available in mode='async' (read the average through state_dict())")
+        plist = list(self._named.values())
+        mine = self._ema_params()
+        err = None
+        if self._no_sync or self._accumulated or self._carry:
+            err = "ema_weights() during gradient accumulation: call step() first"
+        elif self.futures:
+            err = "ema_weights() between backward() and step(): call step() first"
+        elif not all("ema" in self.state[p] for p in mine):
+            err = "ema_weights(): no average has been taken yet (call step() first)"
+        raise_collectively(runtime.world(), self.size, err)
+        averages = {id(p): self.state[p]["ema"] for p in mine}
+        if self.size > 1 and self.mode != "allgather":
+            owners = sorted({r for r in range(self.size) if self._ema_params(r)})
+            posted = [(r, comms.ibroadcast([averages[id(p)] for p in self._ema_params(r)] if self.rank == r else None,
+                                           root=r, level=self.level)) for r in owners]
+            for r, (send, req) in posted:
+                for p, e in zip(self._ema_params(r), comms.irecv1(send, req)):
+                    averages[id(p)] = e
+        saved = [p.detach().clone() for p in plist]
+        self._in_ema_weights = True
+        try:
+            with torch.no_grad():
+                for p in plist:
+                    p.copy_(averages[id(p)].to(device=p.device, dtype=p.dtype))
+            yield
+        finally:
+            with torch.no_grad():
+                for p, q in zip(plist, saved):
+                    p.copy_(q)
+            self._in_ema_weights = False
 
     # -- shared host-engine pieces ---------------------------------------------------------
     def _hyper(self, group) -> Dict[str, Any]:
@@ -710,6 +814,16 @@ class MPI_PS(torch.optim.Optimizer):
 
     def load_state_dict(self, state_dict):
         super().load_state_dict(state_dict)
+        if self._engine is None and self.ema_decay is not None:
+            # torch casts the loaded state to the parameter dtype: keep the saved fp32 average instead
+            params = [p for g in self.param_groups for p in g["params"]]
+            saved = {int(i): st for i, st in state_dict.get("state", {}).items()}
+            have = [torch.is_tensor(saved.get(i, {}).get("ema")) for i in range(len(params))]
+            if any(have) and not all(have):
+                raise ValueError("the checkpoint has a weight average ('ema') for some parameters only")
+            for i, p in enumerate(params):
+                if have[i]:
+                    self.state[p]["ema"] = saved[i]["ema"].to(device=p.device, dtype=torch.float32, copy=True)
         if self._engine is None and self.mode == "sharded" and self.size > 1:
             for p in self._foreign():               # served by another rank: its state is not kept here
                 self.state.pop(p, None)

@@ -139,3 +139,13 @@ class MicroBatchCounter:
         self.n += 1
         self._seen = {key}
         return True
+
+
+def raise_collectively(world, size: int, err) -> None:
+    """A collective refusal: every rank raises ``RuntimeError`` when any rank has a reason ``err`` (the lowest rank's is
+    reported), so no rank is left waiting in a collective that the others never reach.  ``err`` is ``None`` or a message."""
+    every = world.all_gather_object(err) if size > 1 else [err]
+    bad = [(r, e) for r, e in enumerate(every) if e is not None]
+    if bad:
+        r, e = bad[0]
+        raise RuntimeError(e if size == 1 else f"rank {r}: {e}")
